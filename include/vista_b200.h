@@ -42,7 +42,8 @@ int b200v_device_info(int32_t* sm_count, int32_t* cc_major, int32_t* cc_minor);
  *                   v += s_res1*res1[token,n] + s_res2*res2[token,n]
  *   act: 0 none, 1 SiLU, 2 GEGLU (value*gelu_erf(gate); weights/bias pre-permuted so a tile of
  *   tile_n columns holds tile_n/2 value columns followed by their gate columns; N counts the
- *   permuted columns, the output has N/2 columns) — vwm/modules/attention.py:85-93.
+ *   permuted columns, the output has N/2 columns) — vwm/modules/attention.py:85-93,
+ *   3 GELU (erf form, nn.GELU() of the CLIP tower's mlp.c_fc; bias only, fp16 operands and output).
  * ---------------------------------------------------------------------------------------------- */
 typedef struct b200v_gemm_desc {
   const void* a;        /* fp16/bf16 activations */
@@ -278,6 +279,25 @@ int b200v_peer_allreduce_f64(double* data, int32_t n, void* const* windows_dev, 
 int b200v_peer_put(const void* src, int64_t src_pitch, int64_t rows, int64_t row_bytes, void* const* dsts_dev, int64_t dst_pitch,
                    uint32_t* const* flags_dev, int32_t n_dst, uint32_t* counter, uint32_t* ticket, void* stream);
 int b200v_peer_wait(const uint32_t* const* flags_dev, int32_t n, uint32_t* counter, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * CLIP ViT-H/14 image tower of the conditioner (FrozenOpenCLIPImageEmbedder, vwm/modules/encoders/modules.py:251-399;
+ * csrc/clip.cu).  The linear layers, LayerNorms and the token assembly run on b200v_gemm / b200v_layernorm.
+ *   clip_preprocess : x (n,3,H,W) fp32 NCHW in [-1, 1] -> out [n*257, ldo] fp16 patch rows of the patch-embedding GEMM:
+ *       FrozenOpenCLIPImageEmbedder.preprocess (modules.py:293-305) = kornia.geometry.resize to 224 x 224 (bicubic,
+ *       align_corners, Gaussian anti-alias blur when antialias and the image shrinks), (x + 1) / 2, CLIP mean / std;
+ *       row b*257 + 1 + 16 py + px holds patch (py, px) of image b with K index c*196 + 14 dy + dx (the flattening of
+ *       conv1.weight [width, 3, 14, 14]); row b*257 (the class-token slot) and columns 588 .. ldo-1 are zero, so the
+ *       GEMM with a row vector (rv_mod 257) of class embedding + positional embedding yields the tower's input tokens.
+ *       Arithmetic fp32; out_f32 = 1 stores fp32 rows instead of fp16.
+ *   attention_d80   : softmax(Q K^T / sqrt(80)) V per (image, head), head width 80 (the tower's nn.MultiheadAttention);
+ *       q / k / v element (image b, token t, head h, dim d) at q[(b*seq + t)*ld_q + h*80 + d] (column blocks of the fused
+ *       in-proj output), merged-head output likewise.  fp32 softmax and accumulation.
+ * ---------------------------------------------------------------------------------------------- */
+int b200v_clip_preprocess(const float* x, int32_t n, int32_t H, int32_t W, int32_t antialias, void* out, int64_t ldo,
+                          int32_t out_f32, void* stream);
+int b200v_attention_d80(const void* q, int64_t ld_q, const void* k, int64_t ld_k, const void* v, int64_t ld_v, void* out,
+                        int64_t ld_o, int32_t batch, int32_t seq, int32_t heads, void* stream);
 
 /* Layout converters at the boundary: NCHW fp32 <-> token-major (NHWC) fp16/fp32. */
 int b200v_nchw_to_tokens(const float* x, void* out_f16, int64_t ldo, int32_t NB, int32_t C, int32_t H, int32_t W,

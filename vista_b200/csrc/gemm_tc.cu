@@ -1,7 +1,7 @@
 // Tap-GEMM: persistent, warp-specialised wgmma kernel (template tapgemm_kernel<ACT, RV, NRES, GEN, STATS>).
 //   warpgroups 0, 1 : consumers; warpgroup g owns rows 64 g .. 64 g + 63 of the 128-token tile and issues
 //                     wgmma.m64n64k16 (m64n32k16 for a 32-column tail) over the tile_n columns, accumulating in registers;
-//                     then the epilogue (fragment -> smem transpose -> fused bias / row-vector / SiLU / GEGLU / residuals /
+//                     then the epilogue (fragment -> smem transpose -> fused bias / row-vector / SiLU / GEGLU / GELU / residuals /
 //                     GroupNorm statistics -> coalesced stores)
 //   warpgroup 2     : producer; one thread issues the TMA loads (A tile 128 tokens x 64 ch per tap / K-chunk, B tile
 //                     tile_n x 64).  setmaxnreg moves its registers to the consumers (40 / 232 per thread).
@@ -334,6 +334,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             o.x = fmaf(o.x, sa, bs.x); o.y = fmaf(o.y, sa, bs.y); o.z = fmaf(o.z, sa, bs.z); o.w = fmaf(o.w, sa, bs.w);
             if (has_rv) { o.x += rv[i].x; o.y += rv[i].y; o.z += rv[i].z; o.w += rv[i].w; }
             if (act == 1) { o.x = silu_f(o.x); o.y = silu_f(o.y); o.z = silu_f(o.z); o.w = silu_f(o.w); }
+            if (!GEN && act == 3) { o.x = gelu_erf_fast(o.x); o.y = gelu_erf_fast(o.y); o.z = gelu_erf_fast(o.z); o.w = gelu_erf_fast(o.w); }
             if (has_r1) {
               const float2 a = unpack2(u1[i].x, bf16), b = unpack2(u1[i].y, bf16);
               o.x = fmaf(p.s_res1, a.x, o.x); o.y = fmaf(p.s_res1, a.y, o.y);
@@ -391,10 +392,12 @@ extern "C" int b200v_gemm(const b200v_gemm_desc* d, void* stream_) {
   VB_REQUIRE(d->N > 0 && d->N % 8 == 0, "b200v_gemm: N=%d must be a multiple of 8", d->N);
   VB_REQUIRE(d->tile_n >= 32 && d->tile_n <= 256 && d->tile_n % 32 == 0, "b200v_gemm: tile_n=%d invalid", d->tile_n);
   VB_REQUIRE(d->lda % 8 == 0 && d->ldo % 8 == 0, "b200v_gemm: lda/ldo must be multiples of 8");
-  VB_REQUIRE(d->act >= 0 && d->act <= 2, "b200v_gemm: act=%d invalid", d->act);
+  VB_REQUIRE(d->act >= 0 && d->act <= 3, "b200v_gemm: act=%d invalid", d->act);
   VB_REQUIRE(!(d->act == 2 && (d->tile_n % 64 != 0 || d->N % d->tile_n != 0 || d->out_f32)),
              "b200v_gemm: GEGLU needs tile_n %% 64 == 0, N %% tile_n == 0, 16-bit output");
   VB_REQUIRE(!(d->act == 2 && (d->rowvec || d->res1 || d->res2)), "b200v_gemm: GEGLU epilogue takes bias only");
+  VB_REQUIRE(!(d->act == 3 && (d->rowvec || d->res1 || d->res2 || d->bf16 || d->out_f32 || d->stats || getenv("VB_GEMM_GENERIC"))),
+             "b200v_gemm: the GELU epilogue takes bias only, fp16 operands and output (compiled variant)");
   VB_REQUIRE(!d->res1 || d->ld_res1 % 8 == 0, "b200v_gemm: ld_res1 must be a multiple of 8");
   VB_REQUIRE(!d->res2 || d->ld_res2 % 8 == 0, "b200v_gemm: ld_res2 must be a multiple of 8");
   VB_REQUIRE(!d->rowvec || (d->ld_rowvec % 4 == 0 && d->rv_div > 0 && d->rv_mod > 0), "b200v_gemm: bad rowvec args");
@@ -491,10 +494,11 @@ extern "C" int b200v_gemm(const b200v_gemm_desc* d, void* stream_) {
   // Epilogue variant: the common fp16 feature sets are compiled in (no per-element feature tests), everything
   // else (bf16 operands, fp32 output, unusual combinations) takes the generic instantiation.
   using Kern = void (*)(const CUtensorMap, const CUtensorMap, const TGParams);
-  static const Kern kVariants[8] = {tapgemm_kernel<0, false, 0, false>, tapgemm_kernel<0, false, 1, false>,
+  static const Kern kVariants[9] = {tapgemm_kernel<0, false, 0, false>, tapgemm_kernel<0, false, 1, false>,
                                     tapgemm_kernel<0, false, 2, false>, tapgemm_kernel<0, true, 0, false>,
                                     tapgemm_kernel<0, true, 1, false>,  tapgemm_kernel<1, false, 0, false>,
-                                    tapgemm_kernel<2, false, 0, false>, tapgemm_kernel<0, true, 2, true>};
+                                    tapgemm_kernel<2, false, 0, false>, tapgemm_kernel<0, true, 2, true>,
+                                    tapgemm_kernel<3, false, 0, false>};
   int variant = 7;
   if (!d->bf16 && !d->out_f32 && !getenv("VB_GEMM_GENERIC")) {
     const int nres = (d->res1 ? 1 : 0) + (d->res2 ? 1 : 0);
@@ -502,6 +506,7 @@ extern "C" int b200v_gemm(const b200v_gemm_desc* d, void* stream_) {
     else if (d->act == 0 && nres <= 1) variant = 3 + nres;
     else if (d->act == 1 && !d->rowvec && nres == 0) variant = 5;
     else if (d->act == 2) variant = 6;
+    else if (d->act == 3) variant = 8;
   }
   // fused-statistics instantiations: plain, one residual, row vector
   static const Kern kStats[3] = {tapgemm_kernel<0, false, 0, false, true>, tapgemm_kernel<0, false, 1, false, true>,
@@ -510,7 +515,7 @@ extern "C" int b200v_gemm(const b200v_gemm_desc* d, void* stream_) {
   if (vb::first_use_on_device(attr_set)) {
     for (int i = 0; i < 3; ++i)
       VB_CHECK_CUDA(cudaFuncSetAttribute(kStats[i], cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
-    for (int i = 0; i < 8; ++i)
+    for (int i = 0; i < 9; ++i)
       VB_CHECK_CUDA(cudaFuncSetAttribute(kVariants[i], cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
   }
   const long long total = (long long)p.m_tiles * p.n_tiles;

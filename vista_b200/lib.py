@@ -17,7 +17,7 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG_DIR)
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libvista_b200.so")
-SOURCES = ["host.cu", "gemm_tc.cu", "attn_tc.cu", "misc.cu", "glue.cu", "peer.cu"]
+SOURCES = ["host.cu", "gemm_tc.cu", "attn_tc.cu", "misc.cu", "glue.cu", "peer.cu", "clip.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
@@ -129,6 +129,8 @@ SIGNATURES = {
     "b200v_peer_allreduce_f64": [_P, _I32, _P, _I64, _I64, _I32, _I32, _P, _P],
     "b200v_peer_put": [_P, _I64, _I64, _I64, _P, _I64, _P, _I32, _P, _P, _P],
     "b200v_peer_wait": [_P, _I32, _P, _P],
+    "b200v_clip_preprocess": [_P, _I32, _I32, _I32, _I32, _P, _I64, _I32, _P],
+    "b200v_attention_d80": [_P, _I64, _P, _I64, _P, _I64, _P, _I64, _I32, _I32, _I32, _P],
     "b200v_nchw_to_tokens": [_P, _P, _I64, _I32, _I32, _I32, _I32, _P],
     "b200v_tokens_to_nchw": [_P, _I32, _I64, _P, _I32, _I32, _I32, _I32, _P],
 }

@@ -146,7 +146,8 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, taps: Sequence[
          s_acc: float = 1.0, act: int = 0, tile_n: Optional[int] = None, cin: Optional[int] = None,
          stats: Optional[torch.Tensor] = None, h_pad: int = 0) -> torch.Tensor:
     """out = epilogue(tap-GEMM(a, w)).  ``a``: [tokens, >=cin] fp16 view; ``w``: [N, ntaps*cin] fp16;
-    ``geom`` = (W, H, NB) turns on image taps (zero padded); act 2 = GEGLU (out has N/2 columns).
+    ``geom`` = (W, H, NB) turns on image taps (zero padded); act 1 = SiLU, act 2 = GEGLU (out has N/2 columns),
+    act 3 = erf-GELU.
     ``stats`` = partials [tokens/128*4, N, 2] fp32 (may be a column slice of a wider matrix): the epilogue also writes the
     column sums / sums of squares of the output (GroupNorm statistics of the consumer without a pass over the tensor);
     the token tiles are then the 128-consecutive-token ones of stats_box().
@@ -216,6 +217,38 @@ def attention_spatial(q, k, v, out, frames: int, seq: int, heads: int, impl: Opt
                   out.stride(0), frames, seq, heads, _stream()), "b200v_attention_spatial")
     _prof_end()
     _trace("attn_spatial", out)
+    return out
+
+
+def attention_d80(q, k, v, out, batch: int, seq: int, heads: int):
+    """softmax(Q K^T / sqrt(80)) V per (image, head): q / k / v / out are [batch*seq, >= heads*80] fp16 views (column
+    blocks of the CLIP tower's fused in-proj output), the output holds the merged heads."""
+    for t in (q, k, v, out):
+        _rows(t)
+    _count(1)
+    _prof_begin("attn_d80", f"batch={batch} seq={seq} heads={heads}", 4.0 * 80 * heads * batch * seq * seq,
+                2.0 * 4 * batch * seq * heads * 80)
+    _lib.check(_lib.load().b200v_attention_d80(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(),
+                                               v.stride(0), out.data_ptr(), out.stride(0), batch, seq, heads, _stream()),
+               "b200v_attention_d80")
+    _prof_end()
+    _trace("attn_d80", out)
+    return out
+
+
+def clip_preprocess(x, out, antialias: bool = True):
+    """FrozenOpenCLIPImageEmbedder.preprocess + 14x14 patchify: x (n,3,H,W) fp32 in [-1, 1] -> out [n*257, K_pad] fp16
+    (or fp32) patch rows (row b*257 is the zero class-token slot, columns 588.. are zero padding)."""
+    n, c, H, W = x.shape
+    assert c == 3 and x.dtype == torch.float32 and x.is_contiguous()
+    _, ldo = _rows(out)
+    assert out.shape[0] == n * 257 and out.dtype in (torch.float16, torch.float32)
+    _count(1)
+    _prof_begin("other", f"clip_preprocess n={n} {H}x{W}", 0.0, 4.0 * x.numel() + 2.0 * out.numel())
+    _lib.check(_lib.load().b200v_clip_preprocess(x.data_ptr(), n, H, W, int(bool(antialias)), out.data_ptr(), ldo,
+                                                 int(out.dtype == torch.float32), _stream()), "b200v_clip_preprocess")
+    _prof_end()
+    _trace("clip_preprocess", out)
     return out
 
 

@@ -5,7 +5,8 @@
                     later round on the last three latents of the previous one, results stitched into ``samples_z``.
                     The latent bookkeeping between rounds (sample[0] = z[0], samples_z slices, fill_latent) is ONE kernel
                     (``b200v_rollout_advance``) on persistent device buffers, so nothing between two rounds waits for the
-                    host; the reference's decode -> CLIP -> re-encode round trip between rounds is an optional callback.
+                    host; the reference's decode -> CLIP -> re-encode round trip between rounds is an optional callback
+                    (``clip_recondition`` builds it on the native CLIP embedder).
 ``sample_ensemble`` the "reward" path (reward_utils.py:318-337): K samples of the same conditioning with different
                     noise, reward = exp(-mean variance); members are independent, so with a process group they are
                     dealt out over the ranks (replicas, no data-path collective except the final exchange).
@@ -68,6 +69,25 @@ def rollout(engine, cond: Dict, uc: Dict, z: torch.Tensor, num_rounds: int, nois
         return engine.decode_first_stage_u8(samples_z), samples_z
     x = engine.decode_first_stage(samples_z)
     return torch.clamp((x + 1.0) / 2.0, min=0.0, max=1.0), samples_z
+
+
+def clip_recondition(embedder, cond: Dict, uc: Dict, scale_factor: float, n_cond: int = 3, clip_dim: int = 1024) -> Callable:
+    """Opt-in ``recondition=`` callback for ``rollout`` that follows the reference between rounds (sample_utils.py:339-350):
+    decode the tail, embed frame [-3] with ``embedder`` (a vista_b200.clip.FrozenOpenCLIPImagePredictionEmbedder; the frame
+    is repeated over the conditioning rows as get_batch does, :243-244) into ``crossattn[..., :clip_dim]``, and set
+    ``concat`` = sample[[-n_cond]] / scale_factor (the skip_encode rule).  The other crossattn slots and ``vector`` come
+    from ``cond``; ``uc`` is returned as given (its CLIP and concat entries are zero per force_uc_zero_embeddings)."""
+    def recondition(round_idx: int, sample: torch.Tensor, decode_tail: Callable):
+        frames = decode_tail()
+        c = dict(cond)
+        rows = c["crossattn"].shape[0]
+        emb = embedder(frames[[-3]].expand(rows, -1, -1, -1).contiguous())
+        cross = c["crossattn"].clone()
+        cross[..., :clip_dim] = emb.reshape(rows, 1, clip_dim).to(cross.dtype)
+        c["crossattn"] = cross
+        c["concat"] = (sample[[-n_cond]] / scale_factor).expand(c["concat"].shape[0], -1, -1, -1).contiguous()
+        return c, uc
+    return recondition
 
 
 @torch.no_grad()

@@ -420,6 +420,85 @@ def encoder_param_specs(cfg: EncoderConfig = VISTA_ENCODER) -> Dict[str, ParamSp
 
 
 # --------------------------------------------------------------------------------------
+# CLIP image tower of the conditioner (open_clip VisionTransformer under FrozenOpenCLIPImageEmbedder,
+# vwm/modules/encoders/modules.py:251-399; configs/inference/vista.yaml:44-52)
+# --------------------------------------------------------------------------------------
+@dataclass
+class ClipConfig:
+    """open_clip ``VisionTransformer`` shape.  The native tower needs head width 80 (b200v_attention_d80), a LayerNorm
+    width b200v_layernorm supports and widths that are multiples of 64 (the tap-GEMM's K granularity)."""
+    width: int = 1280
+    layers: int = 32
+    head_width: int = 80
+    patch_size: int = 14
+    image_size: int = 224
+    mlp_ratio: float = 4.0
+    embed_dim: int = 1024
+    ln_eps: float = 1e-5
+
+    @property
+    def heads(self) -> int:
+        return self.width // self.head_width
+
+    @property
+    def mlp_width(self) -> int:
+        return int(self.width * self.mlp_ratio)
+
+    @property
+    def grid(self) -> int:
+        return self.image_size // self.patch_size
+
+    @property
+    def tokens(self) -> int:          # class token + patches
+        return self.grid * self.grid + 1
+
+    @property
+    def patch_k(self) -> int:         # 3 * 14 * 14 = 588
+        return 3 * self.patch_size * self.patch_size
+
+    @property
+    def patch_k_pad(self) -> int:     # padded to the GEMM's 64-column K chunks
+        return -(-self.patch_k // 64) * 64
+
+
+VIT_H_14 = ClipConfig()
+
+# what survives ``del model.transformer`` of the open_clip CLIP model besides ``visual`` (modules.py:277): the text
+# tower's leftovers, accepted by load_state_dict and ignored
+CLIP_TEXT_LEFTOVERS = ("token_embedding.weight", "positional_embedding", "ln_final.weight", "ln_final.bias",
+                       "text_projection", "logit_scale")
+
+
+def clip_param_specs(cfg: ClipConfig = VIT_H_14) -> Dict[str, ParamSpec]:
+    """name -> (shape, kind) for open_clip's ``model.visual`` (keys relative to ``visual``)."""
+    C, out = cfg.width, {}
+    out["class_embedding"] = ((C,), "b")
+    out["positional_embedding"] = ((cfg.tokens, C), "b")
+    out["proj"] = ((C, cfg.embed_dim), "w")
+    out["conv1.weight"] = ((C, 3, cfg.patch_size, cfg.patch_size), "w")
+    _norm(out, "ln_pre", C)
+    for i in range(cfg.layers):
+        p = f"transformer.resblocks.{i}"
+        _norm(out, f"{p}.ln_1", C)
+        out[f"{p}.attn.in_proj_weight"] = ((3 * C, C), "w")
+        out[f"{p}.attn.in_proj_bias"] = ((3 * C,), "b")
+        _lin(out, f"{p}.attn.out_proj", C, C)
+        _norm(out, f"{p}.ln_2", C)
+        _lin(out, f"{p}.mlp.c_fc", C, cfg.mlp_width)
+        _lin(out, f"{p}.mlp.c_proj", cfg.mlp_width, C)
+    _norm(out, "ln_post", C)
+    return out
+
+
+def clip_preset(name: str) -> ClipConfig:
+    if name == "vit_h_14":
+        return ClipConfig()
+    if name == "tiny":    # head width 80 kept (the attention kernel), 4 heads, 2 layers, same 1024-wide embedding
+        return ClipConfig(width=320, layers=2)
+    raise KeyError(name)
+
+
+# --------------------------------------------------------------------------------------
 # presets used by tests / oracle / bench
 # --------------------------------------------------------------------------------------
 def unet_preset(name: str) -> UNetConfig:
