@@ -149,48 +149,64 @@ __device__ __forceinline__ void fence_regs(float (&r)[N]) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 
-// D[64 x N] (+)= A[smem desc, 64 x 16] * B[smem desc, 16 x N], both K-major; scale_d = 0 overwrites D.  Accumulator
-// fragment of thread (warp w, lane l) of the warpgroup: d[4 i + e] = D[16 w + l / 4][8 i + 2 (l % 4) + e],
-// d[4 i + 2 + e] = D[16 w + l / 4 + 8][8 i + 2 (l % 4) + e], e in {0, 1}.
-__device__ __forceinline__ void wgmma_m64n64_f16(float (&d)[32], uint64_t da, uint64_t db, int scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "%32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(scale_d));
+// D[64 x N] (+)= A[smem desc, 64 x 16] * B[smem desc, 16 x N], both K-major; scale_d = 0 overwrites D; N any multiple
+// of 32 up to 256, fp16 or bf16 operands.  Accumulator fragment of thread (warp w, lane l) of the warpgroup:
+// d[4 i + e] = D[16 w + l / 4][8 i + 2 (l % 4) + e], d[4 i + 2 + e] = D[16 w + l / 4 + 8][8 i + 2 (l % 4) + e], e in {0, 1}.
+// The descriptors and scale_d are operands %0 .. %2 (read-write only so that they precede the accumulators), so the
+// accumulator list of every N is %3 .. %(N/2 + 2): a prefix of the 16-register blocks below.
+#define VB_R16_0 "%3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18"
+#define VB_R16_1 ", %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34"
+#define VB_R16_2 ", %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50"
+#define VB_R16_3 ", %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66"
+#define VB_R16_4 ", %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82"
+#define VB_R16_5 ", %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98"
+#define VB_R16_6 ", %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114"
+#define VB_R16_7 ", %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127, %128, %129, %130"
+#define VB_D16(b)                                                                                                      \
+  "+f"(d[b + 0]), "+f"(d[b + 1]), "+f"(d[b + 2]), "+f"(d[b + 3]), "+f"(d[b + 4]), "+f"(d[b + 5]), "+f"(d[b + 6]),      \
+      "+f"(d[b + 7]), "+f"(d[b + 8]), "+f"(d[b + 9]), "+f"(d[b + 10]), "+f"(d[b + 11]), "+f"(d[b + 12]),               \
+      "+f"(d[b + 13]), "+f"(d[b + 14]), "+f"(d[b + 15])
+#define VB_WGMMA_SS(N, T, REGS, ...)                                                                                   \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t"                                                      \
+               "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." T "." T " {" REGS "}, %0, %1, p, 1, 1, 0, 0;\n\t}" \
+               : "+l"(da), "+l"(db), "+r"(scale_d), __VA_ARGS__)
+#define VB_WGMMA_SS_T(N, REGS, ...)                                                                                    \
+  do {                                                                                                                 \
+    if constexpr (BF16) VB_WGMMA_SS(N, "bf16", REGS, __VA_ARGS__);                                                     \
+    else VB_WGMMA_SS(N, "f16", REGS, __VA_ARGS__);                                                                     \
+  } while (0)
+template <int N, bool BF16>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, int scale_d) {
+  static_assert(N >= 32 && N <= 256 && N % 32 == 0, "wgmma_ss: N must be a multiple of 32 in [32, 256]");
+  if constexpr (N == 32) VB_WGMMA_SS_T(32, VB_R16_0, VB_D16(0));
+  else if constexpr (N == 64) VB_WGMMA_SS_T(64, VB_R16_0 VB_R16_1, VB_D16(0), VB_D16(16));
+  else if constexpr (N == 96) VB_WGMMA_SS_T(96, VB_R16_0 VB_R16_1 VB_R16_2, VB_D16(0), VB_D16(16), VB_D16(32));
+  else if constexpr (N == 128)
+    VB_WGMMA_SS_T(128, VB_R16_0 VB_R16_1 VB_R16_2 VB_R16_3, VB_D16(0), VB_D16(16), VB_D16(32), VB_D16(48));
+  else if constexpr (N == 160)
+    VB_WGMMA_SS_T(160, VB_R16_0 VB_R16_1 VB_R16_2 VB_R16_3 VB_R16_4, VB_D16(0), VB_D16(16), VB_D16(32), VB_D16(48),
+                  VB_D16(64));
+  else if constexpr (N == 192)
+    VB_WGMMA_SS_T(192, VB_R16_0 VB_R16_1 VB_R16_2 VB_R16_3 VB_R16_4 VB_R16_5, VB_D16(0), VB_D16(16), VB_D16(32),
+                  VB_D16(48), VB_D16(64), VB_D16(80));
+  else if constexpr (N == 224)
+    VB_WGMMA_SS_T(224, VB_R16_0 VB_R16_1 VB_R16_2 VB_R16_3 VB_R16_4 VB_R16_5 VB_R16_6, VB_D16(0), VB_D16(16),
+                  VB_D16(32), VB_D16(48), VB_D16(64), VB_D16(80), VB_D16(96));
+  else
+    VB_WGMMA_SS_T(256, VB_R16_0 VB_R16_1 VB_R16_2 VB_R16_3 VB_R16_4 VB_R16_5 VB_R16_6 VB_R16_7, VB_D16(0), VB_D16(16),
+                  VB_D16(32), VB_D16(48), VB_D16(64), VB_D16(80), VB_D16(96), VB_D16(112));
 }
-
-__device__ __forceinline__ void wgmma_m64n64_bf16(float (&d)[32], uint64_t da, uint64_t db, int scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "%32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-
-__device__ __forceinline__ void wgmma_m64n32_f16(float (&d)[16], uint64_t da, uint64_t db, int scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "%16, %17, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-
-__device__ __forceinline__ void wgmma_m64n32_bf16(float (&d)[16], uint64_t da, uint64_t db, int scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "%16, %17, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
+#undef VB_WGMMA_SS_T
+#undef VB_WGMMA_SS
+#undef VB_D16
+#undef VB_R16_0
+#undef VB_R16_1
+#undef VB_R16_2
+#undef VB_R16_3
+#undef VB_R16_4
+#undef VB_R16_5
+#undef VB_R16_6
+#undef VB_R16_7
 
 __device__ __forceinline__ void wgmma_m64n128_f16(float (&d)[64], uint64_t da, uint64_t db, int scale_d) {
   asm volatile(

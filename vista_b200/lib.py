@@ -17,7 +17,8 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG_DIR)
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libvista_b200.so")
-SOURCES = ["host.cu", "gemm_tc.cu", "attn_tc.cu", "misc.cu", "glue.cu", "peer.cu", "clip.cu"]
+SOURCES = ["host.cu", "gemm_tc.cu", "gemm_tn_32_256.cu", "gemm_tn_64_224.cu", "gemm_tn_96_192.cu", "gemm_tn_128_160.cu",
+           "attn_tc.cu", "misc.cu", "glue.cu", "peer.cu", "clip.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
