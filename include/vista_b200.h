@@ -299,6 +299,32 @@ int b200v_clip_preprocess(const float* x, int32_t n, int32_t H, int32_t W, int32
 int b200v_attention_d80(const void* q, int64_t ld_q, const void* k, int64_t ld_k, const void* v, int64_t ld_v, void* out,
                         int64_t ld_o, int32_t batch, int32_t seq, int32_t heads, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Sinusoidal scalar embedders of the conditioner (ConcatTimestepEmbedderND, vwm/modules/encoders/modules.py:402-425;
+ * csrc/cond.cu).  One launch writes every slot of `table` for all `rows` into column slices of the fp32 output
+ * [rows, ldo] (`vector`, or the action columns of `crossattn`): for slot s and value j of row r,
+ *   out[r, dst_col + j*outdim + k]          = cos(values[r, value_col + j] * freqs[freq_off + k])   k < outdim/2
+ *   out[r, dst_col + j*outdim + outdim/2 + k] = sin(...)                                            (util.py:155-162)
+ * — the "(b d) d2 -> b (d d2)" layout of modules.py:420-422; an odd outdim has a zero last column.  `zero` slots are
+ * written with zeros and read nothing (force_zero_embeddings, modules.py:152-153).  values: fp32 [rows, ld_values];
+ * freqs: fp32 frequency table, computed on the host with the reference's expression.  Full-precision sincosf.
+ * ---------------------------------------------------------------------------------------------- */
+#define B200V_SINUSOID_MAX_SLOTS 16
+typedef struct b200v_sinusoid_slot {
+  int32_t value_col;     /* first column of this slot's values in `values` */
+  int32_t num_features;  /* values per row */
+  int32_t outdim;        /* embedding width per value */
+  int32_t dst_col;       /* first output column */
+  int32_t zero;          /* 1: write zeros */
+  int32_t freq_off;      /* first of the outdim/2 frequencies in `freqs` */
+} b200v_sinusoid_slot;
+typedef struct b200v_sinusoid_table {
+  int32_t n_slots;
+  b200v_sinusoid_slot slot[B200V_SINUSOID_MAX_SLOTS];
+} b200v_sinusoid_table;
+int b200v_sinusoid_embed(const float* values, int64_t ld_values, int32_t rows, const b200v_sinusoid_table* table,
+                         const float* freqs, float* out, int64_t ldo, void* stream);
+
 /* Layout converters at the boundary: NCHW fp32 <-> token-major (NHWC) fp16/fp32. */
 int b200v_nchw_to_tokens(const float* x, void* out_f16, int64_t ldo, int32_t NB, int32_t C, int32_t H, int32_t W,
                          void* stream);

@@ -178,6 +178,10 @@ class FrozenOpenCLIPImagePredictionEmbedder(nn.Module):
         self.open_clip = instantiate_from_config(open_clip_embedding_config)
         self.is_trainable, self.ucg_rate, self.input_key = False, 0.0, None
 
+    def output_shape(self, vid: torch.Tensor):
+        """Shape ``forward(vid)`` returns, without running the tower."""
+        return (vid.shape[0] // self.n_cond_frames * self.n_copies, self.n_cond_frames, self.open_clip.b200_config.embed_dim)
+
     def forward(self, vid: torch.Tensor) -> torch.Tensor:
         z = self.open_clip(vid)
         z = z.reshape(-1, self.n_cond_frames, z.shape[-1])

@@ -2,8 +2,9 @@
 and methods ``sample_utils`` uses (.model, .denoiser, .first_stage_model, .scale_factor, .decode_first_stage,
 .sample, .ema_scope) on top of the B200 executors, plus the SURVEY §8f rows as engine calls (``encode_first_stage`` with
 ``encoder_config: vista_b200.vae.Encoder``, ``rollout``, ``sample_ensemble``, ``decode_first_stage_u8``).  Training is out of
-scope and raises; a conditioner is hosted when a ``conditioner_config`` is given (its ``cond_frames`` embedder can be
-``vista_b200.conditioner.VideoPredictionEmbedderWithEncoder``), not built otherwise."""
+scope and raises; a conditioner is built when a ``conditioner_config`` is given (``vista_b200.conditioner.GeneralConditioner``
+runs every embedder natively, configs/inference/vista_b200_native.yaml), not otherwise; ``condition`` turns a user's
+inputs into ``c`` / ``uc`` with it."""
 from __future__ import annotations
 
 import contextlib
@@ -67,9 +68,11 @@ class DiffusionEngine(nn.Module):
         self.model = wrapper(model, compile_model=False)
         self.denoiser = instantiate_from_config(denoiser_config)
         self.sampler = instantiate_from_config(sampler_config) if sampler_config is not None else None
-        # The conditioner (CLIP / VAE-encoder / sinusoids, encoders/modules.py) is outside the hot path: a user-supplied
-        # one is hosted as is (do_sample calls model.conditioner.get_unconditional_conditioning), none is built here.
+        # The conditioner (CLIP / VAE-encoder / sinusoids, encoders/modules.py): built from conditioner_config when given
+        # (vista_b200.conditioner.GeneralConditioner is the native one; do_sample calls
+        # model.conditioner.get_unconditional_conditioning), none otherwise.  Checkpoint keys `conditioner.*` load into it.
         self._conditioner = instantiate_from_config(conditioner_config) if conditioner_config is not None else None
+        self._register_load_state_dict_pre_hook(self._conditioner_keys)
         if first_stage_config is not None:
             params = first_stage_config.get("params", first_stage_config)
             self.first_stage_model = FirstStage(params["decoder_config"], params.get("encoder_config")
@@ -95,6 +98,44 @@ class DiffusionEngine(nn.Module):
             raise NotImplementedError("no conditioner_config given: the conditioner (CLIP / VAE-encoder / sinusoids) is "
                                       "outside the hot path; pass c / uc dicts, or give a conditioner_config to host")
         return self._conditioner
+
+    @staticmethod
+    def _conditioner_keys(state_dict, prefix, *args):
+        """The reference checkpoint holds the conditioner under `conditioner.*`; this engine keeps it as `_conditioner`."""
+        src, dst = prefix + "conditioner.", prefix + "_conditioner."
+        for k in [k for k in state_dict if k.startswith(src)]:
+            state_dict[dst + k[len(src):]] = state_dict.pop(k)
+
+    @torch.no_grad()
+    def condition(self, value_dict: Dict, num_frames: int, force_uc_zero_embeddings: Optional[List[str]] = None):
+        """(c, uc) from a user's inputs: get_batch + get_condition (sample_utils.py:232-276) on the hosted conditioner —
+        every input repeated over ``num_frames`` rows, the unconditional batch a copy with ``force_uc_zero_embeddings``
+        zeroed, the results trimmed to ``num_frames`` rows (a result with fewer keeps its first row)."""
+        dev = self.device
+        batch = {}
+        for key in {e.input_key for e in self.conditioner.embedders}:
+            if key not in value_dict:
+                continue
+            v = value_dict[key]
+            if key in ("fps", "fps_id", "motion_bucket_id", "cond_aug"):
+                batch[key] = torch.tensor([v]).to(dev).repeat(num_frames)
+            elif key in ("command", "trajectory", "speed", "angle", "goal", "cond_frames", "cond_frames_without_noise"):
+                v = torch.as_tensor(v).to(dev)
+                v = v[None] if key in ("command", "trajectory", "speed", "angle", "goal") else v
+                batch[key] = v.expand((num_frames,) + tuple(v.shape[1:])).contiguous()
+            else:
+                raise NotImplementedError(f"condition: no batch rule for input {key!r} (sample_utils.py:237-247)")
+        batch_uc = {k: v.clone() for k, v in batch.items()}
+        c, uc = self.conditioner.get_unconditional_conditioning(batch, batch_uc=batch_uc,
+                                                                force_uc_zero_embeddings=list(force_uc_zero_embeddings or []))
+        for k in c:
+            if isinstance(c[k], torch.Tensor):
+                c[k], uc[k] = c[k][:num_frames], uc[k][:num_frames]
+                if c[k].shape[0] < num_frames:
+                    c[k] = c[k][[0]]
+                if uc[k].shape[0] < num_frames:
+                    uc[k] = uc[k][[0]]
+        return c, uc
 
     @contextlib.contextmanager
     def ema_scope(self, context=None):          # no-op at inference (diffusion.py:241-255, use_ema False)

@@ -18,7 +18,7 @@ ROOT = os.path.dirname(PKG_DIR)
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libvista_b200.so")
 SOURCES = ["host.cu", "gemm_tc.cu", "gemm_tn_32_256.cu", "gemm_tn_64_224.cu", "gemm_tn_96_192.cu", "gemm_tn_128_160.cu",
-           "attn_tc.cu", "misc.cu", "glue.cu", "peer.cu", "clip.cu"]
+           "attn_tc.cu", "misc.cu", "glue.cu", "peer.cu", "clip.cu", "cond.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
@@ -88,6 +88,20 @@ class GemmDesc(C.Structure):
     ]
 
 
+SINUSOID_MAX_SLOTS = 16
+
+
+class SinusoidSlot(C.Structure):
+    """Mirror of ``b200v_sinusoid_slot`` (include/vista_b200.h)."""
+    _fields_ = [("value_col", C.c_int32), ("num_features", C.c_int32), ("outdim", C.c_int32), ("dst_col", C.c_int32),
+                ("zero", C.c_int32), ("freq_off", C.c_int32)]
+
+
+class SinusoidTable(C.Structure):
+    """Mirror of ``b200v_sinusoid_table``."""
+    _fields_ = [("n_slots", C.c_int32), ("slot", SinusoidSlot * SINUSOID_MAX_SLOTS)]
+
+
 _P, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 
 # name -> argtypes; every function returns int (0 = ok).  Must list every symbol of the header.
@@ -134,6 +148,7 @@ SIGNATURES = {
     "b200v_attention_d80": [_P, _I64, _P, _I64, _P, _I64, _P, _I64, _I32, _I32, _I32, _P],
     "b200v_nchw_to_tokens": [_P, _P, _I64, _I32, _I32, _I32, _I32, _P],
     "b200v_tokens_to_nchw": [_P, _I32, _I64, _P, _I32, _I32, _I32, _I32, _P],
+    "b200v_sinusoid_embed": [_P, _I64, _I32, C.POINTER(SinusoidTable), _P, _P, _I64, _P],
 }
 
 _lib: Optional[C.CDLL] = None

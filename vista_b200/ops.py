@@ -462,6 +462,33 @@ def timestep_embedding(t, out, dim: int, max_period: float = 10000.0):
     return out
 
 
+def sinusoid_embed(values: Optional[torch.Tensor], slots: Sequence[Tuple[int, int, int, int, bool, int]],
+                   freqs: Optional[torch.Tensor], out: torch.Tensor):
+    """Every sinusoidal-embedder slot of one conditioning tensor in one launch (csrc/cond.cu).  out: fp32 [rows, >= cols]
+    (row stride out.stride(0)); values: fp32 [rows, n_values] or None when every slot is zero; slots: (value_col,
+    num_features, outdim, dst_col, zero, freq_off); freqs: fp32 frequency table on the device."""
+    rows, ldo = _rows(out)
+    assert out.dtype == torch.float32 and 0 < len(slots) <= _lib.SINUSOID_MAX_SLOTS
+    if values is not None:
+        _, ldv = _rows(values)
+        assert values.dtype == torch.float32 and values.shape[0] == rows
+    else:
+        ldv = 0
+    assert freqs is None or (freqs.dtype == torch.float32 and freqs.is_contiguous())
+    tab = _lib.SinusoidTable()
+    tab.n_slots = len(slots)
+    for i, (vc, nf, od, dc, zero, fo) in enumerate(slots):
+        s = tab.slot[i]
+        s.value_col, s.num_features, s.outdim, s.dst_col, s.zero, s.freq_off = vc, nf, od, dc, int(bool(zero)), fo
+    _count(1)
+    _prof_begin("other", f"sinusoid_embed rows={rows} slots={len(slots)}", 0.0, 4.0 * rows * out.shape[1])
+    _lib.check(_lib.load().b200v_sinusoid_embed(_ptr(values), ldv, rows, C.byref(tab), _ptr(freqs), out.data_ptr(), ldo,
+                                                _stream()), "b200v_sinusoid_embed")
+    _prof_end()
+    _trace("sinusoid_embed", out)
+    return out
+
+
 def blend_emb(e_plain, e_cond, label, mask, emb, silu_emb):
     rows, dim = e_plain.shape
     _count(1)

@@ -6,7 +6,8 @@
                     The latent bookkeeping between rounds (sample[0] = z[0], samples_z slices, fill_latent) is ONE kernel
                     (``b200v_rollout_advance``) on persistent device buffers, so nothing between two rounds waits for the
                     host; the reference's decode -> CLIP -> re-encode round trip between rounds is an optional callback
-                    (``clip_recondition`` builds it on the native CLIP embedder).
+                    (``clip_recondition`` builds it on the native CLIP embedder, ``conditioner_recondition`` re-runs the
+                    engine's whole conditioner as do_sample does).
 ``sample_ensemble`` the "reward" path (reward_utils.py:318-337): K samples of the same conditioning with different
                     noise, reward = exp(-mean variance); members are independent, so with a process group they are
                     dealt out over the ranks (replicas, no data-path collective except the final exchange).
@@ -87,6 +88,27 @@ def clip_recondition(embedder, cond: Dict, uc: Dict, scale_factor: float, n_cond
         c["crossattn"] = cross
         c["concat"] = (sample[[-n_cond]] / scale_factor).expand(c["concat"].shape[0], -1, -1, -1).contiguous()
         return c, uc
+    return recondition
+
+
+def conditioner_recondition(engine, value_dict: Dict, force_uc_zero_embeddings: Optional[Sequence[str]] = None,
+                            n_cond: int = 3) -> Callable:
+    """Opt-in ``recondition=`` callback for ``rollout`` that re-runs the engine's conditioner between rounds the way
+    sample_utils.py:338-351 does: decoded frame [-n_cond] of the tail -> ``cond_frames_without_noise``,
+    sample[[-n_cond]] / scale_factor -> ``cond_frames``, and ``engine.condition`` with ``skip_encode`` set on the embedders
+    that have it (the latents pass through the cond-frame embedder).  ``value_dict`` is not modified."""
+    def recondition(round_idx: int, sample: torch.Tensor, decode_tail: Callable):
+        vd = dict(value_dict)
+        vd["cond_frames_without_noise"] = decode_tail()[[-n_cond]]
+        vd["cond_frames"] = sample[[-n_cond]] / engine.scale_factor
+        toggled = [e for e in engine.conditioner.embedders if hasattr(e, "skip_encode")]
+        for e in toggled:
+            e.skip_encode = True
+        try:
+            return engine.condition(vd, engine.num_frames, force_uc_zero_embeddings)
+        finally:
+            for e in toggled:
+                e.skip_encode = False
     return recondition
 
 
