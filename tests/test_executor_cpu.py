@@ -711,56 +711,3 @@ def test_peer_memory_sharded_sampler_on_emulated_windows(world):
         assert np.array_equal(out, out2), "second sample on the same state differs"
         r = rel_l2(torch.from_numpy(out), ref)
         assert r < 5e-3, (rank, r)
-
-
-def _gdecode_worker(rank, world, port, q):
-    import os
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    torch.set_num_threads(1)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        import sys
-        sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-        from fake_ops import patched_ops as patched
-        from helpers import decoder_weights as dw, to_t as tt
-        from vista_b200 import synth as sy
-        from vista_b200.sharded import ShardedDecoderRuntime, decode_first_stage_grouped
-        from vista_b200.vae import DecoderRuntime, decode_first_stage
-        cfg, sd = dw("tiny")
-        z = torch.from_numpy(sy.normal(9, "decfs.z", (25, cfg.z_channels, 8, 16), std=0.18215))
-        cache = {}
-        with patched(), torch.no_grad():
-            serial = decode_first_stage(DecoderRuntime(cfg, tt(sd), "cpu"), z)
-            grouped = decode_first_stage_grouped(cfg, lambda g: ShardedDecoderRuntime(cfg, tt(sd), "cpu", group=g), cache, z)
-            again = decode_first_stage_grouped(cfg, lambda g: ShardedDecoderRuntime(cfg, tt(sd), "cpu", group=g), cache, z)
-        groups = cache[("groups", 2)][0]
-        q.put((rank, serial.numpy(), grouped.numpy(), again.numpy(), groups))
-    finally:
-        dist.destroy_process_group()
-
-
-@pytest.mark.parametrize("world", [8, 10])
-def test_grouped_decode_on_emulated_ops(world):
-    """The 2 chunks of a 25-frame clip on two sub-groups of 4 ranks, each frame-sharding its chunk, results broadcast to
-    everyone (8 ranks); 10 ranks: two groups of 4 + two ranks that only receive.  Same frames on every rank, equal to the
-    serial decode up to the halo-correction rounding."""
-    import os
-    import numpy as np
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 39500 + (os.getpid() + 13 * world) % 2000
-    procs = [ctx.Process(target=_gdecode_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = sorted((q.get(timeout=600) for _ in procs), key=lambda t: t[0])
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
-    assert res[0][4] == [list(range(0, 4)), list(range(world // 2, world // 2 + 4))]
-    for rank, serial, grouped, again, _ in res:
-        assert np.array_equal(grouped, res[0][2]), f"rank {rank} holds different frames"
-        assert np.array_equal(grouped, again)
-        r = rel_l2(torch.from_numpy(grouped), torch.from_numpy(serial))
-        assert r < 3e-3, (rank, r)

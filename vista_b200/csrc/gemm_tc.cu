@@ -26,7 +26,7 @@ extern "C" int b200v_gemm(const b200v_gemm_desc* d, void* stream_) {
   VB_REQUIRE(!(d->act == 2 && (d->tile_n % 64 != 0 || d->N % d->tile_n != 0 || d->out_f32)),
              "b200v_gemm: GEGLU needs tile_n %% 64 == 0, N %% tile_n == 0, 16-bit output");
   VB_REQUIRE(!(d->act == 2 && (d->rowvec || d->res1 || d->res2)), "b200v_gemm: GEGLU epilogue takes bias only");
-  VB_REQUIRE(!(d->act == 3 && (d->rowvec || d->res1 || d->res2 || d->bf16 || d->out_f32 || d->stats || getenv("VB_GEMM_GENERIC"))),
+  VB_REQUIRE(!(d->act == 3 && (d->rowvec || d->res1 || d->res2 || d->bf16 || d->out_f32 || d->stats)),
              "b200v_gemm: the GELU epilogue takes bias only, fp16 operands and output (compiled variant)");
   VB_REQUIRE(!d->res1 || d->ld_res1 % 8 == 0, "b200v_gemm: ld_res1 must be a multiple of 8");
   VB_REQUIRE(!d->res2 || d->ld_res2 % 8 == 0, "b200v_gemm: ld_res2 must be a multiple of 8");
@@ -124,7 +124,7 @@ extern "C" int b200v_gemm(const b200v_gemm_desc* d, void* stream_) {
   int variant = d->bf16 ? 12 : 7;
   if (d->stats) {
     variant = 9 + (d->rowvec ? 2 : (d->res1 ? 1 : 0));
-  } else if (!d->bf16 && !d->out_f32 && !getenv("VB_GEMM_GENERIC")) {
+  } else if (!d->bf16 && !d->out_f32) {
     const int nres = (d->res1 ? 1 : 0) + (d->res2 ? 1 : 0);
     if (d->act == 0 && !d->rowvec) variant = nres;
     else if (d->act == 0 && nres <= 1) variant = 3 + nres;

@@ -1055,11 +1055,10 @@ extern "C" int b200v_layernorm(const void* x, int64_t ldx, void* y, int64_t ldy,
   const long long blocks_needed = (tokens + wpb - 1) / wpb;
   const int nv = (C / 8 + 31) / 32;
   const int ad = av_div > 0 ? av_div : 1, am = av_mod > 0 ? av_mod : 1;
-  static const bool ln40 = !(getenv("VB_LN40") && atoi(getenv("VB_LN40")) == 0);
-  if (ln40 && (C == 320 || C == 640 || C == 1280)) {
+  if (C == 320 || C == 640 || C == 1280) {
     // the UNet's three widths: lanes-per-row kernel (gamma / beta in registers, no idle lanes)
     using namespace vb;
-#define VB_LN40_LAUNCH(LPR)                                                                                          \
+#define VB_LAYERNORM40_LAUNCH(LPR)                                                                                   \
   {                                                                                                                  \
     static int per_sm = 0;                                                                                           \
     if (per_sm == 0 && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, layernorm40_kernel<LPR>, 128, 0) !=   \
@@ -1071,10 +1070,10 @@ extern "C" int b200v_layernorm(const void* x, int64_t ldx, void* y, int64_t ldy,
     layernorm40_kernel<LPR><<<(unsigned)blocks, 128, 0, (cudaStream_t)stream>>>(                                     \
         (const __half*)x, ldx, (__half*)y, ldy, tokens, gamma, beta, eps, addvec, ld_addvec, ad, am);                \
   }
-    if (C == 320) VB_LN40_LAUNCH(8)
-    else if (C == 640) VB_LN40_LAUNCH(16)
-    else VB_LN40_LAUNCH(32)
-#undef VB_LN40_LAUNCH
+    if (C == 320) VB_LAYERNORM40_LAUNCH(8)
+    else if (C == 640) VB_LAYERNORM40_LAUNCH(16)
+    else VB_LAYERNORM40_LAUNCH(32)
+#undef VB_LAYERNORM40_LAUNCH
     VB_CHECK_CUDA(cudaGetLastError());
     return 0;
   }

@@ -147,22 +147,14 @@ class DiffusionEngine(nn.Module):
         if not isinstance(dec, VideoDecoder):
             raise NotImplementedError("decode_first_stage needs vista_b200.vae.VideoDecoder as decoder_config.target")
         if getattr(self.model, "frame_sharded", False):     # one clip on several ranks: spread the decode as well
-            import os
             import torch.distributed as dist
             from .vae import _decode_chunks, decode_first_stage_parallel
             group = getattr(self.model, "world_group", None)
             n_chunks = len(_decode_chunks(z.shape[0], self.en_and_decode_n_samples_a_time or z.shape[0], overlap))
-            mode = os.environ.get("VISTA_B200_SHARDED_DECODE", "auto")
-            if mode == "grouped":
-                # opt-in: chunks over sub-groups of <= 4 ranks that frame-shard them (8 ranks: 2 groups x 4 on the 2 chunks)
-                from .sharded import ShardedDecoderRuntime, decode_first_stage_grouped
-                cache = dec.__dict__.setdefault("_grouped_cache", {})
-                return decode_first_stage_grouped(dec.b200_config, lambda g: ShardedDecoderRuntime(dec.b200_config, dec.state_dict(), z.device, group=g),
-                                                  cache, z, self.scale_factor, self.en_and_decode_n_samples_a_time, overlap, world_group=group)
-            # auto: frame-shard the chunks when there are more ranks than chunks — up to 4 ranks, where that path is validated
+            # frame-shard the chunks when there are more ranks than chunks — up to 4 ranks, where that path is validated
             # on hardware; an 8-rank frame chain over NCCL point-to-point timed out in its first hardware run, so larger
             # worlds deal whole chunks out instead
-            if mode == "1" or (mode == "auto" and n_chunks < dist.get_world_size(group) <= 4):
+            if n_chunks < dist.get_world_size(group) <= 4:
                 # more ranks than chunks: shard the FRAMES of every chunk (sharded.ShardedDecoderRuntime)
                 from .sharded import ShardedDecoderRuntime, decode_first_stage_sharded
                 srt = getattr(dec, "_sharded_rt", None)

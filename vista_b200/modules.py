@@ -103,7 +103,7 @@ class _RuntimeOwner:
         import torch.distributed as dist
         world, rank = dist.get_world_size(group), dist.get_rank(group)
         if cfg_split is None:
-            cfg_split = world % 2 == 0 and os.environ.get("VISTA_B200_CFG_SPLIT", "1") != "0"
+            cfg_split = world % 2 == 0
         self.frame_sharded = True
         self.world_group = group          # the group the clip is spread over (engine.decode_first_stage deals chunks over it)
         self.cfg_half, self.pair_group = None, None

@@ -367,8 +367,7 @@ def gather_latent(x_local: torch.Tensor, num_frames: int, group=None) -> torch.T
 # UNet's round-1 path — the temporal GroupNorm's sums are all-reduced, the (3,1,1) convolutions get one-frame halo corrections,
 # the closing 3-tap time mix (AE3DConv, temporal_ae.py:90-97) reads one halo frame of its 3-channel input on each side.
 # Host-side orchestration only.  The engine picks it when there are more ranks than chunks, up to 4 ranks (validated on
-# hardware at 2 and 4: 1.5e-3 against the serial decode at 4, one more fp16 rounding per halo correction; 0.115 s per clip);
-# VISTA_B200_SHARDED_DECODE=1 forces it.
+# hardware at 2 and 4: 1.5e-3 against the serial decode at 4, one more fp16 rounding per halo correction; 0.115 s per clip).
 # ---------------------------------------------------------------------------------------------------------------
 from .vae import DecoderRuntime, _decode_chunks      # noqa: E402  (kept next to its only user)
 
@@ -494,13 +493,9 @@ class ShardedDecoderRuntime(DecoderRuntime):
 
 
 def decode_first_stage_sharded(rt: ShardedDecoderRuntime, z: torch.Tensor, scale_factor: float = 0.18215,
-                               n_samples: Optional[int] = 14, overlap: int = 3, chunk_ids=None, world_group=None,
-                               owners=None) -> torch.Tensor:
+                               n_samples: Optional[int] = 14, overlap: int = 3) -> torch.Tensor:
     """decode_first_stage with the FRAMES of every chunk sharded over the ranks of rt.group; every rank passes the same
-    z and receives the whole clip.  Chunk / overlap rule as in the serial path (vwm/models/diffusion.py:150-180).
-    Grouped mode (decode_first_stage_grouped): rt.group is a SUB-group that decodes only the chunks in ``chunk_ids``; the
-    other chunks arrive by broadcast over ``world_group`` from ``owners[chunk]`` (a global rank of the group that decoded
-    it), and every rank of the world assembles the clip in chunk order with the serial path's arithmetic."""
+    z and receives the whole clip.  Chunk / overlap rule as in the serial path (vwm/models/diffusion.py:150-180)."""
     F_, zc, h, w = z.shape
     n_samples = F_ if n_samples is None else n_samples
     up = 2 ** (len(rt.cfg.ch_mult) - 1)
@@ -510,14 +505,7 @@ def decode_first_stage_sharded(rt: ShardedDecoderRuntime, z: torch.Tensor, scale
     chunks = _decode_chunks(F_, n_samples, overlap)
     if any(nov > n or o0 != f0 for f0, n, o0, nov in chunks):
         raise NotImplementedError("decode_first_stage_sharded: chunks shorter than the overlap")
-    for ci, (f0, n, o0, nov) in enumerate(chunks):
-        if chunk_ids is not None and ci not in chunk_ids:          # another sub-group decodes this chunk
-            chunk = torch.empty(n, rt.cfg.out_ch, H, W, dtype=torch.float32, device=z.device)
-            dist.broadcast(chunk, src=owners[ci], group=world_group)
-            if nov:
-                out[o0:o0 + nov] = 0.5 * (out[o0:o0 + nov] + chunk[:nov])
-            out[o0 + nov:o0 + n] = chunk[nov:]
-            continue
+    for f0, n, o0, nov in chunks:
         rt._set_chunk(n)
         pad = max(b - a for a, b in rt.shards)
         mine = torch.zeros(pad, rt.cfg.out_ch, H, W, dtype=torch.float32, device=z.device)
@@ -533,50 +521,7 @@ def decode_first_stage_sharded(rt: ShardedDecoderRuntime, z: torch.Tensor, scale
         dist.all_gather_into_tensor(gathered, mine, group=rt.group)
         parts = gathered.reshape(rt.world, pad, rt.cfg.out_ch, H, W)
         chunk = torch.cat([parts[r, : b - a] for r, (a, b) in enumerate(rt.shards)], dim=0)
-        if chunk_ids is not None:                                  # hand the chunk to the other sub-groups
-            dist.broadcast(chunk, src=owners[ci], group=world_group)
         if nov:
             out[o0:o0 + nov] = 0.5 * (out[o0:o0 + nov] + chunk[:nov])
         out[o0 + nov:o0 + n] = chunk[nov:]
     return out
-
-
-def decode_groups(world_group, n_chunks: int, max_group: int = 4):
-    """Sub-groups for the grouped decode: the W ranks of `world_group` are cut into min(n_chunks, W // 2) contiguous groups
-    (at most `max_group` ranks each are used: a frame chain that long is what the hardware tests cover); group i decodes
-    chunks i, i + G, ...  Collective: every rank of `world_group` must call it (dist.new_group).  -> (groups as lists of
-    global ranks, process groups, index of this rank's group or None if it sits out)."""
-    ranks = list(range(dist.get_world_size())) if world_group is None else dist.get_process_group_ranks(world_group)
-    W = len(ranks)
-    G = max(1, min(n_chunks, W // 2))
-    per = min(max_group, W // G)
-    groups = [ranks[i * (W // G): i * (W // G) + per] for i in range(G)]
-    pgs = [dist.new_group(g) for g in groups]
-    me = dist.get_rank()
-    mine = next((i for i, g in enumerate(groups) if me in g), None)
-    return groups, pgs, mine
-
-
-def decode_first_stage_grouped(cfg, make_rt, cache: dict, z: torch.Tensor, scale_factor: float = 0.18215,
-                               n_samples: Optional[int] = 14, overlap: int = 3, world_group=None) -> torch.Tensor:
-    """Chunks dealt out over SUB-groups of ranks, each sub-group frame-sharding its chunks (decode_first_stage_sharded on the
-    sub-group): with 8 ranks and the 2 chunks of a 25-frame clip, two groups of 4 decode one chunk each, in parallel.
-    `cfg` = the DecoderConfig, `make_rt(group)` builds the ShardedDecoderRuntime of a sub-group; `cache` keeps groups / runtime across calls.
-    Opt-in (VISTA_B200_SHARDED_DECODE=grouped): the host logic is tested under gloo at 8 ranks, the sub-group path of the
-    decoder has not run on hardware."""
-    F_ = z.shape[0]
-    n_s = F_ if n_samples is None else n_samples
-    chunks = _decode_chunks(F_, n_s, overlap)
-    key = ("groups", len(chunks))
-    if key not in cache:
-        groups, pgs, mine = decode_groups(world_group, len(chunks))
-        cache[key] = (groups, pgs, mine, make_rt(pgs[mine]) if mine is not None else None)
-    groups, pgs, mine, rt = cache[key]
-    G = len(groups)
-    owners = {ci: groups[ci % G][0] for ci in range(len(chunks))}
-    if rt is None:                                   # a rank outside every group still assembles the clip from the broadcasts
-        import types
-        return decode_first_stage_sharded(types.SimpleNamespace(cfg=cfg), z, scale_factor, n_samples, overlap, chunk_ids=set(),
-                                          world_group=world_group, owners=owners)
-    mine_ids = {ci for ci in range(len(chunks)) if ci % G == mine}
-    return decode_first_stage_sharded(rt, z, scale_factor, n_samples, overlap, chunk_ids=mine_ids, world_group=world_group, owners=owners)

@@ -19,7 +19,6 @@ hand-written kernels.  Design points (DESIGN.md has the full list):
 from __future__ import annotations
 
 import math
-import os
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Tuple
 
@@ -37,8 +36,6 @@ class Lin:
     tile_n: int
     geglu: bool = False
 
-
-FUSE_GN_STATS = os.environ.get("VISTA_B200_FUSE_GN", "1") != "0"   # GroupNorm statistics from the producer's epilogue
 
 IN_PAD = 64   # token rows of the network input: 8 channels used, zero padded to one 64-channel K chunk
 
@@ -258,7 +255,7 @@ class UNetRuntime:
     def _fuse_stats(self, B, h, w) -> bool:
         """GroupNorm statistics come out of the producing GEMM's epilogue where the token tiles are runs of 128 consecutive
         tokens (ops.stats_box): 72 x 128 and 36 x 64 of the BASELINE shape, every level of the decoder."""
-        return FUSE_GN_STATS and ops.stats_box(w, h, B) is not None
+        return ops.stats_box(w, h, B) is not None
 
     def _resblock(self, L, x, dst, B, h, w, xp=None, dp=None):
         """xp: column partials of x (None: the statistics of x take their own pass); dp: where to put those of dst."""

@@ -118,8 +118,7 @@ class DecoderRuntime:
         return t
 
     def _fuse_stats(self, T, h, w) -> bool:
-        from .unet import FUSE_GN_STATS
-        return FUSE_GN_STATS and ops.stats_box(w, h, T) is not None
+        return ops.stats_box(w, h, T) is not None
 
     def _resblock(self, L, x, T, h, w, name, xp=None):
         """Returns (output, its GroupNorm column partials or None); xp: those of x."""
@@ -539,33 +538,3 @@ class VideoDecoder(nn.Module):
 
     def get_last_layer(self, skip_time_mix=False, **kwargs):
         return self.conv_out.time_mix_conv.weight if not skip_time_mix else self.conv_out.weight
-
-
-def bench_decode(dcfg: DecoderConfig, rand_sd, dev, T: int, h: int, w: int, reps: int = 1, parallel: bool = False) -> float:
-    """Seconds for one chunked decode of a T-frame clip (warm).  parallel: chunks dealt out over the ranks of the
-    default process group (every rank must call; the caller takes the max over ranks)."""
-    import os
-    sd = rand_sd(decoder_param_specs(dcfg))
-    frame_sharded = parallel and os.environ.get("VISTA_B200_SHARDED_DECODE") == "1"     # force the frame-sharded decode
-    if frame_sharded:
-        from .sharded import ShardedDecoderRuntime, decode_first_stage_sharded
-        rt = ShardedDecoderRuntime(dcfg, sd, dev)
-    else:
-        rt = DecoderRuntime(dcfg, sd, dev)
-    z = torch.randn(T, dcfg.z_channels, h, w, device=dev) * 0.18215
-    if parallel:
-        import torch.distributed as dist
-        dist.broadcast(z, src=0)
-    if frame_sharded:
-        fn = lambda: decode_first_stage_sharded(rt, z)
-    else:
-        fn = (lambda: decode_first_stage_parallel(rt, z)) if parallel else (lambda: decode_first_stage(rt, z))
-    fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / 1e3 / reps
