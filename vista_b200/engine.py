@@ -214,6 +214,12 @@ class DiffusionEngine(nn.Module):
         from .rollout import rollout
         return rollout(self, cond, uc, z, num_rounds, **kwargs)
 
+    def rollout_session(self, value_dict: Dict, z: torch.Tensor, **kwargs):
+        """The same rollout in closed loop (vista_b200/session.py): ``step(action)`` samples one round conditioned on that
+        action and returns its final uint8 frames; ``close()`` returns the last round's final three."""
+        from .session import RolloutSession
+        return RolloutSession(self, value_dict, z, **kwargs)
+
     def sample_ensemble(self, cond: Dict, uc: Dict, z: torch.Tensor, ensemble_size: int = 5, **kwargs):
         """The reward path (reward_utils.py:318-337) -> (reward, members)."""
         from .rollout import sample_ensemble

@@ -221,16 +221,9 @@ def decode_first_stage(rt: DecoderRuntime, z: torch.Tensor, scale_factor: float 
         out8 = torch.empty(F_, h * up, w * up, rt.cfg.out_ch, dtype=torch.uint8, device=z.device)
         chunks = _decode_chunks(F_, n_samples, overlap)
         for ci, (f0, n, o0, nov) in enumerate(chunks):
-            tok = rt.buf("d.z", n * h * w, 8)
-            tok.zero_()
-            ops.nchw_to_tokens(zs[f0:f0 + n].contiguous(), tok, n, zc, h, w)
-            blend = None
-            if nov:
-                blend = torch.zeros(n, dtype=torch.int32, device=z.device)
-                blend[:nov] = 1
             # fp32 is kept only for the frames the NEXT chunk averages with (its first `nov` output frames)
             keep = n if ci + 1 == len(chunks) else max(0, chunks[ci + 1][2] - o0)
-            rt.forward(tok, n, h, w, out, out_frame0=o0, blend=blend, out_u8=out8, keep_f32_from=keep)
+            decode_chunk_u8(rt, zs[f0:f0 + n], out, out8, o0, nov, keep)
         return out8
 
     def run(frames: torch.Tensor, out_frame0: int, n_overlap: int):
@@ -247,6 +240,22 @@ def decode_first_stage(rt: DecoderRuntime, z: torch.Tensor, scale_factor: float 
     for f0, n, o0, nov in _decode_chunks(F_, n_samples, overlap):
         run(zs[f0:f0 + n], o0, nov)
     return out
+
+
+def decode_chunk_u8(rt: DecoderRuntime, zs: torch.Tensor, out: torch.Tensor, out8: torch.Tensor, out_frame0: int,
+                    n_overlap: int, keep_f32_from: int) -> None:
+    """One chunk of the uint8 decode.  zs: the chunk's (n,4,h,w) latents / scale_factor.  Writes out8[out_frame0 + t] for
+    t < n; frames t < n_overlap are averaged with the fp32 frames out[out_frame0 + t] the previous chunk kept; the fp32 of
+    frames t >= keep_f32_from is kept in out[out_frame0 + t] for the next chunk."""
+    n, zc, h, w = zs.shape
+    tok = rt.buf("d.z", n * h * w, 8)
+    tok.zero_()
+    ops.nchw_to_tokens(zs.contiguous(), tok, n, zc, h, w)
+    blend = None
+    if n_overlap:
+        blend = torch.zeros(n, dtype=torch.int32, device=zs.device)
+        blend[:n_overlap] = 1
+    rt.forward(tok, n, h, w, out, out_frame0=out_frame0, blend=blend, out_u8=out8, keep_f32_from=keep_f32_from)
 
 
 # ---------------------------------------------------------------------------------------------------------------
