@@ -75,6 +75,8 @@ def gemm(a, w, out, *, taps=((0, 0),), geom=None, bias=None, rowvec=None, rv_div
         hh = tn // 2
         t = acc.reshape(tokens, N // tn, 2, hh)
         acc = (t[:, :, 0] * F.gelu(t[:, :, 1])).reshape(tokens, N // 2)
+    elif act == 3:                               # erf-GELU
+        acc = F.gelu(acc)
     if res1 is not None:
         acc = acc + s_res1 * _f(res1)
     if res2 is not None:

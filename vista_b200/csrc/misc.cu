@@ -450,7 +450,9 @@ attn_temporal_kernel(const __half* __restrict__ q, long long ld_q, const __half*
   __shared__ __align__(128) uint8_t tiles[kTaWarps][3][32 * 128];   // per warp: Q, K, V tiles of 32 rows x 128 B
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t sQ = smem_u32(tiles[warp][0]), sK = smem_u32(tiles[warp][1]), sV = smem_u32(tiles[warp][2]);
-  // zero the padding rows once (rows >= T are never written afterwards)
+  // zero the tiles once: rows >= T of K and V are never written afterwards, so padded keys score against zeros (and
+  // are masked) and padded V rows add nothing.  The Q tile's rows >= Tq are not reloaded and hold the previous item's
+  // O staging; they only feed S / O rows >= Tq, which are never stored.
   for (int i = lane; i < 3 * 32 * 8; i += 32) reinterpret_cast<uint4*>(tiles[warp][0])[i] = make_uint4(0, 0, 0, 0);
   __syncwarp();
   const long long items = (long long)nb * S * heads;

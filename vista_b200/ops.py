@@ -152,7 +152,14 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, taps: Sequence[
     column sums / sums of squares of the output (GroupNorm statistics of the consumer without a pass over the tensor);
     the token tiles are then the 128-consecutive-token ones of stats_box().
     ``h_pad``: ``a`` holds h_pad extra rows of H before and after the H rows of ``geom`` (halo frames of the frame-sharded
-    (3,1,1) convolution): ``a`` is the extended [(NB (H + 2 h_pad) W), C] tensor, the output has NB H W rows."""
+    (3,1,1) convolution): ``a`` is the extended [(NB (H + 2 h_pad) W), C] tensor, the output has NB H W rows.
+    ``bias`` / ``rowvec`` are fp32; ``res1`` / ``res2`` have the operand dtype whatever the output dtype (the kernel reads
+    them as 16-bit values); GEGLU takes a bias only (no ``s_acc``)."""
+    assert bias is None or bias.dtype == torch.float32, f"gemm: bias must be fp32, got {bias.dtype}"
+    assert rowvec is None or rowvec.dtype == torch.float32, f"gemm: rowvec must be fp32, got {rowvec.dtype}"
+    for r in (res1, res2):
+        assert r is None or r.dtype == a.dtype, f"gemm: residual dtype {r.dtype} != operand dtype {a.dtype}"
+    assert act != 2 or s_acc == 1.0, "gemm: the GEGLU epilogue does not scale by s_acc"
     tokens, lda = _rows(a)
     if h_pad:
         assert geom is not None and tokens == geom[2] * (geom[1] + 2 * h_pad) * geom[0]
