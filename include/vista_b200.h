@@ -49,9 +49,14 @@ typedef struct b200v_gemm_desc {
   const void* a;        /* fp16/bf16 activations */
   int64_t lda;          /* row stride of A in elements (multiple of 8) */
   int64_t tokens;       /* number of A rows = NB*H*W */
-  int32_t a_mode;       /* 0: linear (2-D), 1: image taps (4-D view c,w,h,b with zero padding) */
-  int32_t W, H, NB;     /* a_mode 1: geometry of the view; a_mode 0: ignored */
-  int32_t box_w, box_h, box_b; /* a_mode 1: token tile, box_w*box_h*box_b == 128 */
+  int32_t a_mode;       /* 0: linear (2-D), 1: image taps (4-D view c,w,h,b with zero padding), 2: image taps over the
+                         * nearest-2x upsampled view of A — output pixel (f, y, x) of the NB x 2H x 2W result reads
+                         * A pixel (f, floor((y + dh) / 2), floor((x + dw) / 2)), zero outside; the output has 4 tokens
+                         * rows (token (f * 2H + y) * 2W + x).  The upsampled tensor is never written.  Epilogue: bias
+                         * and fused statistics only (act 0, no rowvec / residuals / s_acc, fp16 operands and output) */
+  int32_t W, H, NB;     /* a_mode 1: geometry of the view; a_mode 2: geometry of A (low resolution); a_mode 0: ignored */
+  int32_t box_w, box_h, box_b; /* a_mode 1 / 2: token tile of A, box_w*box_h*box_b == 128 (a_mode 2: each box makes 4 tiles,
+                                * one per output parity) */
   int32_t cin;          /* channels per tap (multiple of 64) */
   int32_t ntaps;        /* 1..9 */
   int32_t dh[9];        /* tap offsets along h and w */

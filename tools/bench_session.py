@@ -10,10 +10,7 @@ decode); for both, how many chunks the decoder ran; and whether the two paths' b
 
     python tools/bench_session.py [--rounds 4] [--pairs 2] [--height 576] [--width 1024] [--out result.json]
 
-At 576 x 1024 this engine does not fit on one 80 GB H100: after the first round's sampling 34.9 GiB are allocated (weights,
-the UNet executor's buffers, the conditioner), and the decoder's buffers for a 14-frame chunk need more than the 42.8 GiB
-it got before running out.  ``engine.rollout`` with the same re-conditioning stops at the same point.  A smaller frame
-(--height / --width, multiples of 64) runs the same code.
+A smaller frame (--height / --width, multiples of 64) runs the same code.
 """
 import argparse
 import json

@@ -54,9 +54,14 @@ extern "C" int b200v_gemm(const b200v_gemm_desc* d, void* stream_) {
     uint32_t es[2] = {1, 1};
     if (encode_tmap_16bit(&tmA, d->a, 2, dims, strides, box, es, d->bf16)) return 3;
   } else {
+    VB_REQUIRE(d->a_mode == 1 || d->a_mode == 2, "b200v_gemm: a_mode=%d invalid", d->a_mode);
+    const long long out_tokens = d->a_mode == 2 ? 4ll * d->tokens : d->tokens;
     VB_REQUIRE(d->W > 0 && d->H > 0 && d->NB > 0 && (long long)d->W * d->H * d->NB == d->tokens &&
-                   d->tokens < (1ll << 31) - 256,
-               "b200v_gemm: W*H*NB != tokens (or >= 2^31)");
+                   out_tokens < (1ll << 31) - 256,
+               "b200v_gemm: W*H*NB != tokens (or output tokens >= 2^31)");
+    VB_REQUIRE(d->a_mode == 1 || (d->h_pad == 0 && d->act == 0 && !d->rowvec && !d->res1 && !d->res2 && !d->bf16 &&
+                                  !d->out_f32 && d->s_acc == 1.0f),
+               "b200v_gemm: the upsampling mode (a_mode 2) takes bias and fused statistics only, fp16 in and out");
     VB_REQUIRE(d->box_w > 0 && d->box_h > 0 && d->box_b > 0 && d->box_w * d->box_h * d->box_b == 128,
                "b200v_gemm: box_w*box_h*box_b must be 128");
     p.W = d->W; p.H = d->H; p.NB = d->NB;
@@ -64,7 +69,7 @@ extern "C" int b200v_gemm(const b200v_gemm_desc* d, void* stream_) {
     p.tiles_w = (d->W + p.BW - 1) / p.BW;
     p.tiles_h = (d->H + p.BH - 1) / p.BH;
     const int tiles_b = (d->NB + p.BB - 1) / p.BB;
-    p.m_tiles = p.tiles_w * p.tiles_h * tiles_b;
+    p.m_tiles = p.tiles_w * p.tiles_h * tiles_b * (d->a_mode == 2 ? 4 : 1);
     VB_REQUIRE(d->h_pad >= 0 && d->h_pad <= 4, "b200v_gemm: h_pad=%d out of range", d->h_pad);
     const uint64_t He = (uint64_t)d->H + 2ull * d->h_pad;     // rows of H in memory (halo rows before and after)
     uint64_t dims[4] = {(uint64_t)d->cin, (uint64_t)d->W, He, (uint64_t)d->NB};
@@ -113,8 +118,12 @@ extern "C" int b200v_gemm(const b200v_gemm_desc* d, void* stream_) {
     VB_REQUIRE(d->stats_ld >= d->stats_col0 + d->N && d->stats_col0 % 4 == 0 && d->stats_ld % 4 == 0 &&
                    (reinterpret_cast<uintptr_t>(d->stats) & 15) == 0,
                "b200v_gemm: bad stats_ld / stats_col0 / alignment");
-    VB_REQUIRE(d->a_mode == 0 || (p.BB == 1 && d->W % p.BW == 0 && d->H % p.BH == 0 && (p.BW == d->W || p.BH == 1)),
-               "b200v_gemm: fused statistics need token tiles of 128 consecutive tokens (box %d x %d x %d on %d x %d)",
+    // a_mode 2: a tile is one parity of one low-resolution box, and the tiles of a frame (4 H W / 128 of them) are
+    // consecutive when boxes tile the frame exactly: groupnorm_from_partials reads a frame's partials as one block
+    VB_REQUIRE(d->a_mode == 0 || (p.BB == 1 && d->W % p.BW == 0 && d->H % p.BH == 0 &&
+                                  (d->a_mode == 2 || p.BW == d->W || p.BH == 1)),
+               "b200v_gemm: fused statistics need token tiles of 128 consecutive tokens, or boxes that tile each frame "
+               "in upsampling mode (box %d x %d x %d on %d x %d)",
                p.BW, p.BH, p.BB, d->W, d->H);
   }
 

@@ -7,7 +7,9 @@
 //                     tile_n x 64).  setmaxnreg moves its registers to the consumers (40 / 232 per thread).
 // The shared-memory ring (up to 8 stages) runs ahead of the consumers across tile boundaries, so the loads of tile i+1
 // overlap the epilogue of tile i.  The 3x3 / (3,1,1) convolutions are implicit GEMMs: the A tile of every tap is a
-// shifted 4-D TMA box of the token-major activation, zero padding comes from TMA OOB fill.
+// shifted 4-D TMA box of the token-major activation, zero padding comes from TMA OOB fill.  a_mode 2 convolves the
+// nearest-2x upsampled view of a low-resolution tensor without materialising it: a tile is one low-resolution box and
+// one output parity (py, px); within it upsampling is a shift, so every tap is again one shifted box of the low tensor.
 // gemm_tn_*.cu instantiate the kernels of two tile widths each (so that they compile in parallel); gemm_tc.cu holds
 // the launcher.
 #pragma once
@@ -116,9 +118,12 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const uint32_t tx = (uint32_t)(kABytes + TN * 128);
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int m_blk = tile / p.n_tiles, n_blk = tile - m_blk * p.n_tiles;
-        const int tw = m_blk % p.tiles_w;
-        const int th = (m_blk / p.tiles_w) % p.tiles_h;
-        const int tb = m_blk / (p.tiles_w * p.tiles_h);
+        const int up = p.a_mode == 2;
+        const int box = up ? (m_blk >> 2) : m_blk;     // a_mode 2: four output parities per low-resolution box
+        const int px = up ? (m_blk & 1) : 0, py = up ? ((m_blk >> 1) & 1) : 0;
+        const int tw = box % p.tiles_w;
+        const int th = (box / p.tiles_w) % p.tiles_h;
+        const int tb = box / (p.tiles_w * p.tiles_h);
         const int w0 = tw * p.BW, h0 = th * p.BH, b0 = tb * p.BB;
         const int n0 = n_blk * TN;
         for (int kc = 0; kc < KC; ++kc) {
@@ -128,10 +133,13 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           const int tap = kc / p.kc_per_tap;
           const int c0 = (kc - tap * p.kc_per_tap) * 64;
           mbar_expect_tx(&full[stage], tx);
+          // a_mode 2: upsampled pixel 2 j + px shifted by d reads low-resolution pixel j + floor((px + d) / 2)
+          const int dw = up ? ((px + p.dw[tap]) >> 1) : p.dw[tap];
+          const int dh = up ? ((py + p.dh[tap]) >> 1) : p.dh[tap];
           if (p.a_mode == 0)
             tma_load_2d(sA, &tmA, &full[stage], c0, w0);
           else
-            tma_load_4d(sA, &tmA, &full[stage], c0, w0 + p.dw[tap], h0 + p.dh[tap], b0);
+            tma_load_4d(sA, &tmA, &full[stage], c0, w0 + dw, h0 + dh, b0);
           tma_load_2d(sB, &tmB, &full[stage], kc * 64, n0);
           if (++stage == p.nstages) {
             stage = 0;
@@ -205,14 +213,18 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       token_own = m_blk * 128 + r_own;
       valid_own = token_own < p.tokens;
     } else {
-      const int tw = m_blk % p.tiles_w;
-      const int t2 = m_blk / p.tiles_w;
+      const int up = p.a_mode == 2;
+      const int box = up ? (m_blk >> 2) : m_blk;
+      const int tw = box % p.tiles_w;
+      const int t2 = box / p.tiles_w;
       const int th = t2 % p.tiles_h;
       const int tb = t2 / p.tiles_h;
       const int ww = r_own & (p.BW - 1), hh = (r_own >> p.bw_sh) & (p.BH - 1), bb = r_own >> (p.bw_sh + p.bh_sh);
       const int w = tw * p.BW + ww, h = th * p.BH + hh, b = tb * p.BB + bb;
       valid_own = (w < p.W) && (h < p.H) && (b < p.NB);
-      token_own = (b * p.H + h) * p.W + w;
+      // a_mode 2: output pixel (2 h + py, 2 w + px) of the (2 H) x (2 W) frame
+      token_own = up ? ((2 * (b * p.H + h) + ((m_blk >> 1) & 1)) * 2 * p.W + 2 * w + (m_blk & 1))
+                     : (b * p.H + h) * p.W + w;
     }
     if (!valid_own) token_own = 0;
     // phase-B row i of this lane = 8 i + rsub (of the warp's 32)

@@ -119,6 +119,15 @@ def stats_box(W: int, H: int, NB: int) -> Optional[Tuple[int, int, int]]:
     return None
 
 
+def upsample_stats_box(W: int, H: int) -> Optional[Tuple[int, int, int]]:
+    """Low-resolution box (box_w, box_h, 1) of the upsampling tap-GEMM (``gemm(..., upsample=True)``) that tiles every
+    frame exactly — what fused statistics need there; None if the geometry has none."""
+    for bw in (128, 64, 32, 16, 8, 4, 2, 1):
+        if W % bw == 0 and H % (128 // bw) == 0:
+            return (bw, 128 // bw, 1)
+    return None
+
+
 def pick_tile_n(N: int, geglu: bool = False) -> int:
     """tile_n <= 256 (multiple of 32, of 64 for GEGLU) minimising the time of one row of n-tiles under a cost model
     with a fixed per-tile part (pipeline fill, epilogue set-up) and a part linear in the width above 128 columns,
@@ -144,7 +153,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, taps: Sequence[
          res1: Optional[torch.Tensor] = None, s_res1: float = 1.0,
          res2: Optional[torch.Tensor] = None, s_res2: float = 1.0,
          s_acc: float = 1.0, act: int = 0, tile_n: Optional[int] = None, cin: Optional[int] = None,
-         stats: Optional[torch.Tensor] = None, h_pad: int = 0) -> torch.Tensor:
+         stats: Optional[torch.Tensor] = None, h_pad: int = 0, upsample: bool = False) -> torch.Tensor:
     """out = epilogue(tap-GEMM(a, w)).  ``a``: [tokens, >=cin] fp16 view; ``w``: [N, ntaps*cin] fp16;
     ``geom`` = (W, H, NB) turns on image taps (zero padded); act 1 = SiLU, act 2 = GEGLU (out has N/2 columns),
     act 3 = erf-GELU.
@@ -153,6 +162,9 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, taps: Sequence[
     the token tiles are then the 128-consecutive-token ones of stats_box().
     ``h_pad``: ``a`` holds h_pad extra rows of H before and after the H rows of ``geom`` (halo frames of the frame-sharded
     (3,1,1) convolution): ``a`` is the extended [(NB (H + 2 h_pad) W), C] tensor, the output has NB H W rows.
+    ``upsample``: the taps run over the nearest-2x upsampled view of ``a`` (``geom`` is the geometry of ``a``; ``out`` and
+    ``stats`` cover the 4x as many tokens of NB x 2H x 2W), without writing the upsampled tensor; bias and ``stats``
+    are the only epilogue features, and the statistics boxes are upsample_stats_box()'s.
     ``bias`` / ``rowvec`` are fp32; ``res1`` / ``res2`` have the operand dtype whatever the output dtype (the kernel reads
     them as 16-bit values); GEGLU takes a bias only (no ``s_acc``)."""
     assert bias is None or bias.dtype == torch.float32, f"gemm: bias must be fp32, got {bias.dtype}"
@@ -170,14 +182,20 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, taps: Sequence[
     assert K == ntaps * cin and w.is_contiguous()
     d = _lib.GemmDesc()
     d.a, d.lda, d.tokens = a.data_ptr(), lda, tokens
+    out_tokens = 4 * tokens if upsample else tokens
     if geom is None:
-        assert ntaps == 1
+        assert ntaps == 1 and not upsample
         d.a_mode = 0
     else:
-        d.a_mode = 1
+        d.a_mode = 2 if upsample else 1
         d.W, d.H, d.NB = geom
         assert geom[0] * geom[1] * geom[2] == tokens
-        d.box_w, d.box_h, d.box_b = pick_box(*geom) if stats is None else stats_box(*geom)
+        if upsample and stats is not None:
+            box = upsample_stats_box(geom[0], geom[1])
+            assert box is not None, f"gemm: no box tiles the frames of {geom} for fused statistics"
+        else:
+            box = pick_box(*geom) if stats is None else stats_box(*geom)
+        d.box_w, d.box_h, d.box_b = box
     d.cin, d.ntaps = cin, ntaps
     for i, (dh, dw) in enumerate(taps):
         d.dh[i], d.dw[i] = dh, dw
@@ -197,13 +215,15 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, taps: Sequence[
     if stats is not None:      # [tokens/128*4, >= N, 2] fp32 view (possibly a column slice of a wider partial matrix)
         assert stats.dtype == torch.float32 and stats.dim() == 3 and stats.shape[2] == 2 and stats.stride(2) == 1 \
             and stats.stride(1) == 2 and stats.stride(0) % 2 == 0 and stats.shape[1] >= (N // 2 if act == 2 else N)
-        assert stats.shape[0] >= -(-tokens // 128) * 4
+        assert stats.shape[0] >= -(-out_tokens // 128) * 4
         d.stats, d.stats_ld, d.stats_col0 = stats.data_ptr(), stats.stride(0) // 2, 0
+    assert not upsample or out.shape[0] >= out_tokens
     d.h_pad = h_pad
     _count()
     n_out = N // 2 if act == 2 else N
-    _prof_begin("gemm", f"M={tokens} N={N} K={K} taps={ntaps} act={act}", 2.0 * tokens * N * K,
-                2.0 * tokens * cin + 2.0 * N * K + out.element_size() * tokens * n_out
+    _prof_begin("gemm", f"M={out_tokens} N={N} K={K} taps={ntaps} act={act}{' up2x' if upsample else ''}",
+                2.0 * out_tokens * N * K,
+                2.0 * tokens * cin + 2.0 * N * K + out.element_size() * out_tokens * n_out
                 + (2.0 * tokens * n_out if res1 is not None else 0) + (2.0 * tokens * n_out if res2 is not None else 0))
     _lib.check(_lib.load().b200v_gemm(C.byref(d), _stream()), "b200v_gemm")
     _prof_end()

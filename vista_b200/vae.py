@@ -14,7 +14,7 @@ the stated tolerance is in tests/test_decoder_gpu.py.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -25,8 +25,116 @@ from .spec import DecoderConfig, DecResBlockSpec, build_decoder_plan, decoder_pa
 from .unet import Lin
 from .weights import conv_weight_to_taps
 
+_SCRATCH_ALIGN = 4096      # byte alignment of every role in the decoder's arena (TMA needs 16)
+
+
+def _fuses(T: int, h: int, w: int) -> bool:
+    """Whether the decoder's convolutions at this geometry write their output's GroupNorm partials (ops.stats_box)."""
+    return ops.stats_box(w, h, T) is not None
+
+
+class ScratchPlan(NamedTuple):
+    """The decoder's scratch for one (T, h, w): ``roles`` maps each role to (byte offset, bytes) in one arena of ``total``
+    bytes; ``uses`` lists every view DecoderRuntime.forward takes, in order, as (role, shape, dtype, first op, last op):
+    the view lives from the op that writes it to the last op that reads it.  Roles whose views are never live at the same
+    op may share storage."""
+    roles: Dict[str, Tuple[int, int]]
+    uses: List[Tuple[str, Tuple[int, ...], torch.dtype, int, int]]
+    total: int
+
+
+def _decoder_scratch_uses(cfg: DecoderConfig, T: int, h: int, w: int):
+    """Replays DecoderRuntime.forward's scratch traffic op by op: the role (and shape) every op writes and the views it
+    reads.  Must follow forward / _resblock / _attn; the CPU executor tests run the decoder on this plan."""
+    uses, step = [], [0]
+    f16, f32 = torch.float16, torch.float32
+
+    def op(reads, *writes):
+        for u in reads:
+            if u is not None:
+                u[4] = step[0]
+        out = [None if wr is None else [wr[0], wr[1], wr[2] if len(wr) > 2 else f16, step[0], step[0]] for wr in writes]
+        uses.extend(u for u in out if u is not None)
+        step[0] += 1
+        return out
+
+    def part(role, M, Cc, fuse):
+        return ("part." + role, (-(-M // 128) * 4, Cc, 2), f32) if fuse else None
+
+    def resblock(rb: DecResBlockSpec, x, xp, h, w, name):
+        M, fuse, co = T * h * w, _fuses(T, h, w), rb.cout
+        a1, = op([x, xp], ("d.a1", (M, rb.cin)))
+        h1, p1 = op([a1], ("d.h1", (M, co)), part("d.h1", M, co, fuse))
+        a2, = op([h1, p1], ("d.a2", (M, co)))
+        xs = op([x], ("d.xs", (M, co)))[0] if rb.has_skip else x
+        xsp, p2 = op([a2, xs], ("d.xsp", (M, co)), part("d.xsp", M, co, fuse))
+        a3, = op([xsp, p2], ("d.a1", (M, co)))
+        h2, p1 = op([a3], ("d.h1", (M, co)), part("d.h1", M, co, fuse))
+        a4, = op([h2, p1], ("d.a2", (M, co)))
+        return op([a4, xsp], (name, (M, co)), part(name, M, co, fuse))
+
+    def attn(x, xp, h, w, Cc):
+        M, hw = T * h * w, h * w
+        xn, = op([x, xp], ("d.a1", (M, Cc)))
+        q, = op([xn], ("d.q", (M, Cc)))
+        k, = op([xn], ("d.k", (M, Cc)))
+        # the per-frame loop: V^T, S, P and O are all live until O is complete
+        _, _, _, o = op([xn, q, k], ("d.vT", (Cc, hw)), ("d.s", (hw, hw), f32), ("d.p", (hw, hw)), ("d.o", (M, Cc)))
+        return op([o, x], ("d.attn_y", (M, Cc)), part("d.attn_y", M, Cc, _fuses(T, h, w)))
+
+    plan = build_decoder_plan(cfg)
+    x, = op([], ("d.in", (T * h * w, plan.block_in)))
+    x, xp = resblock(plan.mid[0], x, None, h, w, "d.r0")
+    x, xp = attn(x, xp, h, w, plan.block_in)
+    x, xp = resblock(plan.mid[1], x, xp, h, w, "d.r1")
+    for blocks, up, ch in plan.levels:
+        for bi, rb in enumerate(blocks):
+            x, xp = resblock(rb, x, xp, h, w, f"d.r{bi % 2}")
+        if up is not None:
+            fuse = _fuses(T, 2 * h, 2 * w) and ops.upsample_stats_box(w, h) is not None
+            h, w = 2 * h, 2 * w
+            x, xp = op([x], ("d.upc", (T * h * w, ch)), part("d.upc", T * h * w, ch, fuse))
+    M = T * h * w
+    a, = op([x, xp], ("d.a1", (M, plan.final_ch)))
+    y, = op([a], ("d.y", (M, 8), f32))
+    op([y])
+    return [tuple(u) for u in uses]
+
+
+def decoder_scratch_plan(cfg: DecoderConfig, T: int, h: int, w: int) -> ScratchPlan:
+    """Scratch of DecoderRuntime.forward for T frames of h x w latents: every role sized once for its largest view, and
+    placed first-fit (largest role first) at the lowest offset clear of every role it is live together with at some op."""
+    size: Dict[str, int] = {}
+    live: Dict[str, list] = {}
+    uses = _decoder_scratch_uses(cfg, T, h, w)
+    for role, shape, dtype, first, last in uses:
+        n = dtype.itemsize
+        for s in shape:
+            n *= s
+        size[role] = max(size.get(role, 0), -(-n // _SCRATCH_ALIGN) * _SCRATCH_ALIGN)
+        live.setdefault(role, []).append((first, last))
+
+    def together(r1, r2):
+        return any(a0 <= b1 and b0 <= a1 for a0, a1 in live[r1] for b0, b1 in live[r2])
+
+    roles: Dict[str, Tuple[int, int]] = {}
+    for role in sorted(size, key=lambda r: (-size[r], r)):
+        off = 0
+        for s, e in sorted((roles[o][0], roles[o][0] + roles[o][1]) for o in roles if together(role, o)):
+            if off + size[role] <= s:
+                break
+            off = max(off, e)
+        roles[role] = (off, size[role])
+    return ScratchPlan(roles, uses, max(o + n for o, n in roles.values()))
+
 
 class DecoderRuntime:
+    # forward's scratch: one arena laid out by decoder_scratch_plan (roles: set while forward runs; the encoder and the
+    # frame-sharded decoder keep per-name buffers, buf())
+    _arena: Optional[torch.Tensor] = None
+    _arena_key: Optional[Tuple[int, int, int]] = None
+    _roles: Optional[Dict[str, Tuple[int, int]]] = None
+
     def __init__(self, cfg: DecoderConfig, sd: Dict[str, torch.Tensor], device):
         self.cfg, self.dev = cfg, torch.device(device)
         self.plan = build_decoder_plan(cfg)
@@ -90,7 +198,18 @@ class DecoderRuntime:
         self.tmix_b = self._f32("conv_out.time_mix_conv.bias")
 
     # ------------------------------------------------------------------ helpers
+    def _scratch(self, role, shape, dtype):
+        """View of ``role``'s storage in the planned arena (inside forward)."""
+        off, size = self._roles[role]
+        n = dtype.itemsize
+        for s in shape:
+            n *= s
+        assert n <= size, f"decoder scratch: {role} {shape} exceeds its planned {size} bytes"
+        return self._arena[off:off + n].view(dtype).view(*shape)
+
     def buf(self, name, rows, cols, dtype=torch.float16):
+        if self._roles is not None:
+            return self._scratch(name, (rows, cols), dtype)
         key = (name, rows, cols, dtype)
         t = self._bufs.get(key)
         if t is None:
@@ -111,6 +230,8 @@ class DecoderRuntime:
         return ops.groupnorm_apply(x, y, T, hw, norm[0], norm[1], silu, stats, fps, self.cfg.num_groups)
 
     def part(self, name: str, tokens: int, cols: int) -> torch.Tensor:
+        if self._roles is not None:        # every partial the kernels read was written before (whole-frame tiles)
+            return self._scratch("part." + name, (-(-tokens // 128) * 4, cols, 2), torch.float32)
         key = ("part." + name, tokens, cols)
         t = self._bufs.get(key)
         if t is None:
@@ -118,7 +239,13 @@ class DecoderRuntime:
         return t
 
     def _fuse_stats(self, T, h, w) -> bool:
-        return ops.stats_box(w, h, T) is not None
+        return _fuses(T, h, w)
+
+    def _upsample_in_gemm(self) -> bool:
+        """The up-convolutions read the low-resolution tensor (tap-GEMM a_mode 2) on CUDA, the only device the kernels
+        run on.  A runtime on another device only runs on the host-executor tests' CPU emulation of the operators, which
+        covers upsample2x and the image-tap GEMM but not the upsampling mode: there the 2x upsample is materialised."""
+        return self.dev.type == "cuda"
 
     def _resblock(self, L, x, T, h, w, name, xp=None):
         """Returns (output, its GroupNorm column partials or None); xp: those of x."""
@@ -181,6 +308,21 @@ class DecoderRuntime:
             self.gn_ws = ops.GNWorkspace(self.dev)
         up_total = 2 ** (len(cfg.ch_mult) - 1)
         self.gn_ws.reserve(ops.groupnorm_scratch(T, h * w * up_total * up_total, cfg.num_groups))
+        if self._arena_key != (T, h, w):
+            plan = decoder_scratch_plan(cfg, T, h, w)
+            if self._arena is None or self._arena.numel() < plan.total:
+                # nothing captures the decoder's launches: the old arena can go back to the allocator (stream-ordered)
+                self._arena = None
+                self._arena = torch.empty(plan.total, dtype=torch.uint8, device=self.dev)
+            self._arena_key, self._arena_roles = (T, h, w), plan.roles
+        self._roles = self._arena_roles
+        try:
+            return self._forward(z_tokens, T, h, w, out, out_frame0, blend, skip_frames, out_u8, keep_f32_from)
+        finally:
+            self._roles = None
+
+    def _forward(self, z_tokens, T, h, w, out, out_frame0, blend, skip_frames, out_u8, keep_f32_from):
+        cfg = self.cfg
         M = T * h * w
         x = ops.conv3x3_small_cin(z_tokens, cfg.z_channels, self.conv_in_w, self.conv_in_b,
                                   self.buf("d.in", M, self.plan.block_in), T, h, w)
@@ -191,10 +333,15 @@ class DecoderRuntime:
             for bi, rb in enumerate(blocks):
                 x, xp = self._resblock(self.res[rb.prefix], x, T, h, w, f"d.r{bi % 2}", xp)
             if up is not None:
-                xu = ops.upsample2x(x, self.buf("d.up", T * 4 * h * w, ch), T, h, w, ch)
+                fuse = self._fuse_stats(T, 2 * h, 2 * w) and ops.upsample_stats_box(w, h) is not None
+                xp = self.part("d.upc", T * 4 * h * w, ch) if fuse else None
+                upc = self.buf("d.upc", T * 4 * h * w, ch)
+                if self._upsample_in_gemm():    # nearest-2x upsample + 3x3 conv in one launch, reading x at low resolution
+                    x = self.gemm(x, self.ups[up], upc, taps=ops.TAPS_3X3, geom=(w, h, T), upsample=True, stats=xp)
+                else:
+                    xu = ops.upsample2x(x, torch.empty(T * 4 * h * w, ch, dtype=x.dtype, device=self.dev), T, h, w, ch)
+                    x = self.gemm(xu, self.ups[up], upc, taps=ops.TAPS_3X3, geom=(2 * w, 2 * h, T), stats=xp)
                 h, w = 2 * h, 2 * w
-                xp = self.part("d.upc", T * h * w, ch) if self._fuse_stats(T, h, w) else None
-                x = self.gemm(xu, self.ups[up], self.buf("d.upc", T * h * w, ch), taps=ops.TAPS_3X3, geom=(w, h, T), stats=xp)
         M = T * h * w
         a = self._gn(x, self.buf("d.a1", M, self.plan.final_ch), T, h * w, self.norm_out, 1e-6, self.norm_out_idx, part=xp)
         y = self.gemm(a, self.out_conv, self.buf("d.y", M, 8, torch.float32), taps=ops.TAPS_3X3, geom=(w, h, T))
