@@ -216,7 +216,8 @@ class DiffusionEngine(nn.Module):
 
     def rollout_session(self, value_dict: Dict, z: torch.Tensor, **kwargs):
         """The same rollout in closed loop (vista_b200/session.py): ``step(action)`` samples one round conditioned on that
-        action and returns its final uint8 frames; ``close()`` returns the last round's final three."""
+        action and returns its final uint8 frames; ``close()`` returns the last round's final three; ``score(candidates)``
+        rates actions for the next round with the ensemble reward, and ``fork()`` copies the session."""
         from .session import RolloutSession
         return RolloutSession(self, value_dict, z, **kwargs)
 

@@ -8,9 +8,13 @@ final; frames 22 n + 22 .. 22 n + 24 are averaged with chunk 2 n + 2, so their r
 the first of them is the decoded frame ``do_sample`` re-embeds with CLIP between rounds (sample_utils.py:340-343), the
 raw output of chunk 2 n + 1.  N rounds cost 2 N chunk decodes, against 3 N - 1 for ``engine.rollout`` (N - 1 decodes of
 the tail for the re-conditioning, then the whole clip).
+
+Because that frame is carried, ``score`` samples the next round from the session's state without a decode: it conditions
+each candidate action as ``step`` would, samples an ensemble and rates it with ``reward_utils.do_sample``'s reward.
 """
 from __future__ import annotations
 
+import copy
 from typing import Dict, Optional, Sequence
 
 import torch
@@ -33,7 +37,10 @@ class RolloutSession:
 
     ``value_dict``: what ``engine.condition`` takes.  ``z``: the encoded clip (T, 4, h, w), as ``engine.rollout`` takes it.
     ``action`` of ``step``: a dict of ``ACTION_KEYS`` merged into ``value_dict`` for that round only, or None to keep the
-    previous round's action."""
+    previous round's action.
+
+    For a planner: ``score(candidates)`` rates actions for the next round with the ensemble reward without advancing the
+    session, and ``fork()`` copies the session for a look-ahead over several rounds."""
 
     def __init__(self, engine, value_dict: Dict, z: torch.Tensor, force_uc_zero_embeddings: Optional[Sequence[str]] = None,
                  initial_cond_indices: Sequence[int] = (0,), n_cond: int = 3):
@@ -68,6 +75,27 @@ class RolloutSession:
         """The latents of the rounds so far, laid out as ``engine.rollout``'s ``samples_z``."""
         return self._samples_z
 
+    @staticmethod
+    def _check_action(action: Dict):
+        unknown = sorted(set(action) - set(ACTION_KEYS))
+        if unknown:
+            raise ValueError(f"rollout_session: {unknown} are not action keys {ACTION_KEYS}")
+
+    def _round_inputs(self, action: Dict):
+        """-> (cond, uc, cond_frame, cond_mask): the sampler's inputs for the next round under ``action``.  Round 0 is
+        conditioned on the clip under the initial mask; a later round re-runs the conditioner on the last sample and the
+        carried frames, and is conditioned on the filled latents under the prediction mask.  Reads the session's state and
+        changes none of it."""
+        eng, r = self.engine, self.rounds
+        vd = dict(self.value_dict)
+        vd.update(action)
+        if r == 0:
+            cond, uc = eng.condition(vd, _T, self.uc_keys)
+            return cond, uc, self.z, self._init_mask
+        # the decoded frame do_sample re-embeds is the first carried frame: decode_tail()[[-n_cond]]
+        cond, uc = conditioner_recondition(eng, vd, self.uc_keys, self.n_cond)(r, self._sample, lambda: self._carry)
+        return cond, uc, self._filled.clone(), self._pred_mask
+
     @torch.no_grad()
     def step(self, action: Optional[Dict] = None, noise: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Sample the next round -> its (T - n_cond, H, W, 3) uint8 frames, final.  ``noise``: the round's sampler noise
@@ -75,29 +103,74 @@ class RolloutSession:
         if self._closed:
             raise RuntimeError("rollout_session: step() after close()")
         if action is not None:
-            unknown = sorted(set(action) - set(ACTION_KEYS))
-            if unknown:
-                raise ValueError(f"rollout_session: {unknown} are not action keys {ACTION_KEYS}")
+            self._check_action(action)
             self._action = dict(action)
         eng, z, n, r = self.engine, self.z, self.n_cond, self.rounds
-        vd = dict(self.value_dict)
-        vd.update(self._action)
-        if r == 0:
-            cond, uc = eng.condition(vd, _T, self.uc_keys)
-        else:
-            # the decoded frame do_sample re-embeds is the first carried frame: decode_tail()[[-n_cond]]
-            cond, uc = conditioner_recondition(eng, vd, self.uc_keys, n)(r, self._sample, lambda: self._carry)
+        cond, uc, cond_frame, cond_mask = self._round_inputs(self._action)
         x = torch.randn_like(z) if noise is None else noise.to(z.device, torch.float32).clone().contiguous()
         self._samples_z = torch.cat([self._samples_z, z.new_zeros((_T if r == 0 else _T - n,) + tuple(z.shape[1:]))])
+        sample = eng.sampler(self._den, x, cond, uc=uc, cond_frame=cond_frame, cond_mask=cond_mask)
         if r == 0:
-            sample = eng.sampler(self._den, x, cond, uc=uc, cond_frame=z, cond_mask=self._init_mask)
             ops.rollout_advance(sample, z, self._samples_z, self._filled, 0, 0, n)
         else:
-            sample = eng.sampler(self._den, x, cond, uc=uc, cond_frame=self._filled.clone(), cond_mask=self._pred_mask)
             ops.rollout_advance(sample, None, self._samples_z, self._filled, r * (_T - n), n, n)
         self._sample = sample
         self.rounds += 1
         return self._decode(r)
+
+    @torch.no_grad()
+    def score(self, candidates: Sequence[Optional[Dict]], ensemble_size: int = 5, num_steps: int = 10,
+              noises: Optional[Sequence[torch.Tensor]] = None, seed: int = 0, sampler=None):
+        """Score candidate actions for the next round with the ensemble reward of ``reward_utils.do_sample``
+        (reward_utils.py:318-337) -> (rewards (K,) fp32, members (K, E, T, 4, h, w) fp32), E = ``ensemble_size``.
+
+        Candidate k is sampled E times as the next ``step(candidates[k])`` would sample its round — same conditioning,
+        conditioning frames and mask — but with ``num_steps`` steps, ``sampler`` (default ``engine.sampler``) and member
+        e's noise.  In round 0, member frame 0 is then set to z[0], so round 0 is ``engine.sample_ensemble`` on the same
+        conditioning.  The reward is exp(-mean unbiased variance) over the members, on all T frames (``ops.ensemble_reward``);
+        the re-imposed conditioning frames add no variance.
+
+        ``candidates``: action dicts of ``ACTION_KEYS``, None for the session's current action.  ``noises``: E tensors
+        (T, 4, h, w), member e's noise for every candidate; by default drawn from a generator seeded with ``seed`` on z's
+        device, so the rewards of two candidates differ by their actions only and the global RNG is not drawn from.  The
+        session is not changed: a session that scores samples the same rounds as one that does not."""
+        if self._closed:
+            raise RuntimeError("rollout_session: score() after close()")
+        if isinstance(candidates, dict) or len(candidates) == 0:
+            raise ValueError("rollout_session: score() takes a non-empty list of candidate actions")
+        if not 2 <= ensemble_size <= 64:
+            raise ValueError(f"rollout_session: ensemble_size must be in [2, 64] (the reward kernel's limit), "
+                             f"got {ensemble_size}")
+        for a in candidates:
+            if a is not None:
+                self._check_action(a)
+        z = self.z
+        if noises is None:
+            g = torch.Generator(device=z.device).manual_seed(seed)
+            noises = [torch.randn(z.shape, generator=g, dtype=torch.float32, device=z.device) for _ in range(ensemble_size)]
+        elif len(noises) != ensemble_size or any(tuple(nz.shape) != tuple(z.shape) for nz in noises):
+            raise ValueError(f"rollout_session: noises must be {ensemble_size} tensors of shape {tuple(z.shape)}, got "
+                             f"{[tuple(nz.shape) for nz in noises]}")
+        smp = self.engine.sampler if sampler is None else sampler
+        members = z.new_empty((len(candidates), ensemble_size) + tuple(z.shape))
+        for k, a in enumerate(candidates):
+            cond, uc, cond_frame, cond_mask = self._round_inputs(self._action if a is None else a)
+            for e in range(ensemble_size):
+                x = noises[e].to(z.device, torch.float32).clone().contiguous()
+                members[k, e] = smp(self._den, x, cond, uc=uc, cond_frame=cond_frame, cond_mask=cond_mask,
+                                    num_steps=num_steps)
+            if self.rounds == 0:
+                members[k, :, 0] = z[0]                     # reward_utils.py:324
+        rewards = torch.stack([ops.ensemble_reward(list(members[k]))[1] for k in range(len(candidates))])
+        return rewards, members
+
+    def fork(self) -> "RolloutSession":
+        """A copy of the session that shares the engine: stepping either one afterwards leaves the other as it was."""
+        new = copy.copy(self)
+        new.value_dict, new._action, new.uc_keys = dict(self.value_dict), dict(self._action), list(self.uc_keys)
+        new._samples_z, new._filled = self._samples_z.clone(), self._filled.clone()
+        new._sample, new._carry, new._tail = (None if t is None else t.clone() for t in (self._sample, self._carry, self._tail))
+        return new
 
     def _decode(self, r: int) -> torch.Tensor:
         """Chunks 2 r and 2 r + 1 of the batch decode, with the arguments decode_first_stage(..., u8=True) gives them."""
