@@ -37,6 +37,9 @@ FAMILY = {
     "norm": Family(8.0, 2.0, "fp32 statistics over n elements, then one rounding of the store"),
     # __expf (ex2.approx, relative ~2^-22) and an fp32 sum over the row, one rounding of the store
     "softmax": Family(8.0, 2.0, "approximate exp and an fp32 row sum, then one rounding of the store"),
+    # a fixed, short chain of fp32 operations per element (sampler step, time mix, embeddings): eps counts its roundings
+    # (and the documented ulp errors of rsqrtf / logf / expf / cosf / sinf), derived next to each operation's reference
+    "elementwise": Family(1.0, 2.0, "a few fp32 operations per element, each rounding counted in eps, then the store"),
 }
 
 
@@ -335,14 +338,14 @@ def check_stats(stats, ref, err_bound, name):
 # ==================================================================================================================
 # Attention
 # ==================================================================================================================
-def attention_reference(q, k, v, p_normalised: bool):
-    """fp64 softmax(q k^T / 8) v over the last two dims and its magnitude for the P rounding term (FAMILY['attn'],
-    eps = 2 * 2^-12): P.|V| for the relative half-ulp of every weight, plus 2^-13 sum|V| / d for the absolute 2^-25 of a
-    weight in fp16's subnormal range.  ``p_normalised``: the kernel rounds the normalised weights (temporal, d = 1);
-    otherwise it rounds exp(s - running max) <= 1 and divides by the row sum afterwards (spatial, d = l = sum exp(s - max),
-    the fp64 row sum)."""
+def attention_reference(q, k, v, p_normalised: bool, scale: float = 0.125):
+    """fp64 softmax(q k^T * scale) v over the last two dims (scale 1/8 for head dim 64) and its magnitude for the P
+    rounding term (FAMILY['attn'], eps = 2 * 2^-12): P.|V| for the relative half-ulp of every weight, plus 2^-13 sum|V| / d
+    for the absolute 2^-25 of a weight in fp16's subnormal range.  ``p_normalised``: the kernel rounds the normalised
+    weights (temporal, d = 1); otherwise it rounds exp(s - running max) <= 1 and divides by the row sum afterwards
+    (spatial and CLIP, d = l = sum exp(s - max), the fp64 row sum)."""
     q, k, v = q.double(), k.double(), v.double()
-    s = q @ k.transpose(-1, -2) * 0.125
+    s = q @ k.transpose(-1, -2) * scale
     e = torch.exp(s - s.max(-1, keepdim=True).values)
     l = e.sum(-1, keepdim=True)
     p = e / l

@@ -606,8 +606,9 @@ conv3x3_small_cin_kernel(const __half* __restrict__ x, int cin, const float* __r
       if (hh >= 0 && hh < H && ww >= 0 && ww < W)
         h8_to_f(__ldg(reinterpret_cast<const uint4*>(x + ((b * H + hh) * W + ww) * 8)), f);
     }
+    // channels >= cin are not staged: a NaN / Inf there must not reach the sum through a zero weight (NaN * 0 = NaN)
 #pragma unroll
-    for (int c = 0; c < 8; ++c) patch[t][tap * 8 + c] = f[c];
+    for (int c = 0; c < 8; ++c) patch[t][tap * 8 + c] = c < cin ? f[c] : 0.f;
   }
   __syncthreads();
   for (int n = threadIdx.x; n < cout; n += blockDim.x) {

@@ -433,6 +433,11 @@ def layernorm(x, y, gamma, beta, eps: float = 1e-5, addvec=None, av_div: int = 1
 
 
 def conv3x3_small_cin(x8, cin: int, w, bias, out, NB: int, H: int, W: int):
+    """3x3 convolution (padding 1) of x8 [NB*H*W, 8] fp16 (channels >= cin ignored) with fp32 w [cout, cin, 3, 3] into
+    out [NB*H*W, >= cout] fp16.  The kernel has no row-stride argument: it reads x8 as rows of exactly 8 halves."""
+    _, ldx = _rows(x8)
+    assert x8.dtype == torch.float16 and ldx == 8, \
+        f"conv3x3_small_cin: x8 must be fp16 rows of stride 8, got {x8.dtype} with row stride {ldx}"
     _count(1)
     _prof_begin("other", "conv3x3_small_cin", 0.0, 0.0)
     _lib.check(_lib.load().b200v_conv3x3_small_cin(x8.data_ptr(), cin, w.data_ptr(), _ptr(bias), out.data_ptr(),
