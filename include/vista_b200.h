@@ -336,6 +336,24 @@ int b200v_nchw_to_tokens(const float* x, void* out_f16, int64_t ldo, int32_t NB,
 int b200v_tokens_to_nchw(const void* x, int32_t x_is_f32, int64_t ldx, float* out, int32_t NB, int32_t C, int32_t H,
                          int32_t W, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Camera frames in (sample.py:174-201, load_img; csrc/ingest/ingest.cu).
+ *   frames_u8_resize : T uint8 RGB frames (NHWC, src + t*frame_stride + y*row_stride + 3*x) -> out fp32 (T, 3, out_h,
+ *       out_w) = Image.crop((crop_x, crop_y, crop_x + crop_w, crop_y + crop_h)).resize((out_w, out_h), LANCZOS), then
+ *       ToTensor and x * 2 - 1 (u8 / 255.0f correctly rounded, * 2, - 1), bit for bit Pillow's 8-bit resampler.  Per
+ *       axis the host's tables (vista_b200/ingest.py lanczos_tables): bounds [out][2] = (first input index within the
+ *       crop, count), weights [out][ksize] int32 in 22-bit fixed point.  A pass whose size is unchanged is skipped, as
+ *       Pillow skips it, and its tables may be NULL.  The horizontal pass runs first, over the cropped rows
+ *       [y_first, y_first + y_rows) the vertical pass reads (all crop_h rows when the height is unchanged), into
+ *       scratch (T, y_rows, out_w, 3) uint8 (unused, may be NULL, when the width is unchanged).  Two launches, no
+ *       allocation.
+ * ---------------------------------------------------------------------------------------------- */
+int b200v_frames_u8_resize(const uint8_t* src, int64_t frame_stride, int64_t row_stride, int32_t T, int32_t src_h,
+                           int32_t src_w, int32_t crop_x, int32_t crop_y, int32_t crop_w, int32_t crop_h, int32_t out_h,
+                           int32_t out_w, const int32_t* xbounds, const int32_t* xweights, int32_t xksize,
+                           const int32_t* ybounds, const int32_t* yweights, int32_t yksize, int32_t y_first,
+                           int32_t y_rows, uint8_t* scratch, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

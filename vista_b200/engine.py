@@ -221,6 +221,60 @@ class DiffusionEngine(nn.Module):
         from .session import RolloutSession
         return RolloutSession(self, value_dict, z, **kwargs)
 
+    @torch.no_grad()
+    def frames_from_u8(self, frames: torch.Tensor, height: int = 576, width: int = 1024) -> torch.Tensor:
+        """sample.py's load_img (sample.py:174-201) on decoded RGB frames: uint8 (T, Hs, Ws, 3), on the host or a device,
+        -> (T, 3, height, width) fp32 in [-1, 1] on the engine's device, ``torch.equal`` to load_img's tensors for the
+        same pixels (centre crop, PIL LANCZOS resize, ToTensor, ``* 2 - 1``; vista_b200/ingest.py).  A host tensor is
+        copied to the device as uint8."""
+        from . import ingest
+        ingest.check_frames(frames, height, width)
+        dev = self.device
+        if dev.type != "cuda":
+            raise RuntimeError("frames_from_u8 runs on the CUDA kernels of csrc/ingest/ingest.cu; move the engine to a GPU")
+        return ingest.frames_u8_resize(frames.to(dev), height, width)
+
+    @torch.no_grad()
+    def rollout_session_from_frames(self, frames: torch.Tensor, n_conds: int = 1, cond_aug: float = 0.0,
+                                    action: Optional[Dict] = None, force_uc_zero_embeddings: Optional[List[str]] = None,
+                                    height: int = 576, width: int = 1024, cond_aug_noise: Optional[torch.Tensor] = None,
+                                    encode_noise: Optional[torch.Tensor] = None):
+        """A rollout session started from camera frames, as sample.py does it (sample.py:222-253 and the head of
+        sample_utils.do_sample): frames [0, n_conds) through ``frames_from_u8``; a value dict of
+        sample_utils.init_embedder_options, the first frame as ``cond_frames_without_noise``, that frame plus
+        ``cond_aug * cond_aug_noise`` as ``cond_frames``, ``cond_aug`` and the action keys of ``action``; the frames encoded
+        with ``encode_first_stage``; ``initial_cond_indices = range(n_conds)``.
+
+        Only the conditioning frames [0, n_conds) reach a session: the sampler reads ``z`` under the initial mask,
+        ``rollout_advance`` and ``score`` read z[0].  So only those frames are resized and encoded, and ``z`` is zero on
+        the other frames.  ``frames``: uint8 (>= n_conds, Hs, Ws, 3).  ``cond_aug_noise``: (1, 3, height, width), by
+        default drawn with ``torch.randn_like``.  ``encode_noise``: the posterior noise, (>= n_conds, 4, h, w) of which
+        frames [0, n_conds) are used; by default drawn by ``encode_first_stage``."""
+        from . import ingest
+        from .session import ACTION_KEYS
+        if not isinstance(n_conds, int) or not 1 <= n_conds <= self.num_frames:
+            raise ValueError(f"n_conds must be in [1, {self.num_frames}], got {n_conds}")
+        ingest.check_frames(frames, height, width, min_frames=n_conds)
+        action = dict(action or {})
+        unknown = sorted(set(action) - set(ACTION_KEYS))
+        if unknown:
+            raise ValueError(f"rollout_session_from_frames: {unknown} are not action keys {ACTION_KEYS}")
+        img = self.frames_from_u8(frames[:n_conds], height, width)
+        value_dict = ingest.embedder_options({e.input_key for e in self.conditioner.embedders})
+        cond_img = img[0:1]
+        noise = torch.randn_like(cond_img) if cond_aug_noise is None else cond_aug_noise.to(img.device, torch.float32)
+        value_dict["cond_frames_without_noise"] = cond_img
+        value_dict["cond_aug"] = cond_aug
+        value_dict["cond_frames"] = cond_img + cond_aug * noise
+        value_dict.update(action)
+        if encode_noise is not None:
+            encode_noise = encode_noise[:n_conds].to(img.device, torch.float32).contiguous()
+        zc = self.encode_first_stage(img, noise=encode_noise)
+        z = zc.new_zeros((self.num_frames,) + tuple(zc.shape[1:]))
+        z[:n_conds] = zc
+        return self.rollout_session(value_dict, z, force_uc_zero_embeddings=force_uc_zero_embeddings,
+                                    initial_cond_indices=list(range(n_conds)))
+
     def sample_ensemble(self, cond: Dict, uc: Dict, z: torch.Tensor, ensemble_size: int = 5, **kwargs):
         """The reward path (reward_utils.py:318-337) -> (reward, members)."""
         from .rollout import sample_ensemble

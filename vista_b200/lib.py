@@ -18,7 +18,7 @@ ROOT = os.path.dirname(PKG_DIR)
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libvista_b200.so")
 SOURCES = ["host.cu", "gemm_tc.cu", "gemm_tn_32_256.cu", "gemm_tn_64_224.cu", "gemm_tn_96_192.cu", "gemm_tn_128_160.cu",
-           "attn_tc.cu", "misc.cu", "glue.cu", "peer.cu", "clip.cu", "cond.cu"]
+           "attn_tc.cu", "misc.cu", "glue.cu", "peer.cu", "clip.cu", "cond.cu", "ingest/ingest.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
@@ -34,7 +34,7 @@ def _stale() -> bool:
     if not os.path.isfile(LIB_PATH):
         return True
     t = os.path.getmtime(LIB_PATH)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(ROOT, "include", "vista_b200.h")]
+    deps = [os.path.join(d, f) for d, _, files in os.walk(CSRC) for f in files] + [os.path.join(ROOT, "include", "vista_b200.h")]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
@@ -49,6 +49,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     objs = []
     for src in SOURCES:
         obj = os.path.join(objdir, src.replace(".cu", ".o"))
+        os.makedirs(os.path.dirname(obj), exist_ok=True)
         objs.append(obj)
         cmd = [nvcc] + NVCC_FLAGS + ["-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
@@ -149,6 +150,8 @@ SIGNATURES = {
     "b200v_nchw_to_tokens": [_P, _P, _I64, _I32, _I32, _I32, _I32, _P],
     "b200v_tokens_to_nchw": [_P, _I32, _I64, _P, _I32, _I32, _I32, _I32, _P],
     "b200v_sinusoid_embed": [_P, _I64, _I32, C.POINTER(SinusoidTable), _P, _P, _I64, _P],
+    "b200v_frames_u8_resize": [_P, _I64, _I64, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _I32, _P, _P,
+                               _I32, _I32, _I32, _P, _P, _P],
 }
 
 _lib: Optional[C.CDLL] = None

@@ -610,6 +610,31 @@ def rollout_advance(sample, z0, samples_z, filled, dst_frame0: int, src_frame0: 
     return samples_z
 
 
+def frames_u8_resize(frames, box, out, xtab, ytab, y_first: int, y_rows: int, scratch=None):
+    """load_img's crop + LANCZOS resize + ToTensor + ``* 2 - 1`` (csrc/ingest/ingest.cu): frames (T, Hs, Ws, 3) uint8 with
+    adjacent channels, box = (left, top, crop_w, crop_h) -> out (T, 3, H, W) fp32.  xtab / ytab = (bounds, weights, ksize)
+    on the device (vista_b200.ingest.device_tables), None for an axis whose size is unchanged; scratch holds
+    (T, y_rows, W, 3) uint8 when the width changes."""
+    T, Hs, Ws, _ = frames.shape
+    _, _, H, W = out.shape
+    left, top, cw, ch = box
+    assert frames.dtype == torch.uint8 and frames.stride(3) == 1 and frames.stride(2) == 3
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.shape[:2] == (T, 3)
+    assert scratch is None or (scratch.dtype == torch.uint8 and scratch.numel() >= T * y_rows * W * 3)
+    xb, xw, xk = xtab if xtab is not None else (None, None, 0)
+    yb, yw, yk = ytab if ytab is not None else (None, None, 0)
+    _count(1 + (xtab is not None))
+    mid = T * y_rows * W * 3 if xtab is not None else 0
+    _prof_begin("other", f"frames_u8_resize T={T} {Ws}x{Hs}->{W}x{H}", 0.0, float(T * ch * cw * 3 + 2 * mid + out.numel() * 4))
+    _lib.check(_lib.load().b200v_frames_u8_resize(frames.data_ptr(), frames.stride(0), frames.stride(1), T, Hs, Ws, left, top,
+                                                  cw, ch, H, W, _ptr(xb), _ptr(xw), xk, _ptr(yb), _ptr(yw), yk, y_first,
+                                                  y_rows, _ptr(scratch), out.data_ptr(), _stream()),
+               "b200v_frames_u8_resize")
+    _prof_end()
+    _trace("frames_u8_resize", out)
+    return out
+
+
 _reward_ws = {}
 
 
