@@ -213,6 +213,11 @@ int b200v_blend_emb(const float* e_plain, const float* e_cond, const float* labe
  *            and, when `final`, re-imposes the conditioning frames  (sampling.py:122-123)
  * sigma values are read from the device array `sigmas` at index *step_idx (device int); update
  * increments *step_idx so that a captured CUDA graph can be replayed for every step.
+ *   update_2m: D as in update; then, with {a, b, c, e} = coefs[4 * *step_idx ..] (DPM-Solver++(2M),
+ *            Lu et al. 2022, arXiv 2211.01095, Algorithm 2; a = s'/s, b = expm1(-h), h = ln(s/s'),
+ *            c = 1 + 1/(2r), e = 1/(2r), r = h_prev/h; c = 1, e = 0 on a first-order row):
+ *            x = a*x - b*(c*D - e*d_prev); d_prev = D             (d_prev is not read when e == 0)
+ *            and, when `final`, re-imposes the conditioning frames
  * ---------------------------------------------------------------------------------------------- */
 int b200v_sampler_prepare(float* x, const float* cond_frame, const float* mask,
                           const float* concat_u /* uncond rows (T,4,h,w) or NULL = zeros */,
@@ -222,6 +227,11 @@ int b200v_sampler_prepare(float* x, const float* cond_frame, const float* mask,
 int b200v_sampler_update(float* x, const float* net_out /* [2T*h*w, ld_net] fp32 token-major, 4 channels used */,
                          int64_t ld_net, const float* cond_frame, const float* mask, const float* scales /* [T] */, const float* sigmas, int32_t* step_idx,
                          int32_t num_steps, int32_t T, int32_t h, int32_t w, void* stream);
+int b200v_sampler_update_2m(float* x, const float* net_out /* as in b200v_sampler_update */, int64_t ld_net,
+                            const float* cond_frame, const float* mask, const float* scales /* [T] */,
+                            const float* coefs /* [num_steps, 4] fp32 {a, b, c, e}, 16-byte aligned */,
+                            float* d_prev /* (T,4,h,w) fp32, the previous step's D */, const float* sigmas,
+                            int32_t* step_idx, int32_t num_steps, int32_t T, int32_t h, int32_t w, void* stream);
 
 /* VAE decoder helpers.
  *   softmax_rows : fp32 scores -> fp16 probabilities, one row per block (mid.attn_1 single-head d=512

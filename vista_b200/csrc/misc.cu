@@ -803,11 +803,15 @@ __global__ void sampler_prepare_kernel(float* __restrict__ x, const float* __res
   *reinterpret_cast<uint4*>(unet_in + (((long long)T + t) * hw + pix) * ld_in) = f_to_h8(cu);
 }
 
+// <false>: the Euler step.  <true>: the DPM-Solver++(2M) step x = a x - b (c D - e D_prev), D_prev = D, with
+// {a, b, c, e} = coefs[step] from the host (vista_b200.diffusion.dpmpp2m_coefficients); e == 0 marks a first-order
+// row, on which D_prev is not read (it is uninitialised at a sample's first step).
+template <bool kMultistep>
 __global__ void sampler_update_kernel(float* __restrict__ x, const float* __restrict__ net,
                                       const float* __restrict__ cond_frame, const float* __restrict__ mask,
                                       const float* __restrict__ scales, const float* __restrict__ sigmas,
                                       const int* __restrict__ step_idx, int num_steps, int T, int h, int w,
-                                      long long ld_net) {
+                                      long long ld_net, const float4* __restrict__ coefs, float* __restrict__ d_prev) {
   const int step = *step_idx;
   const float sigma = sigmas[step], sigma_next = sigmas[step + 1];
   const float c_skip = 1.0f / (sigma * sigma + 1.0f);
@@ -830,8 +834,17 @@ __global__ void sampler_update_kernel(float* __restrict__ x, const float* __rest
     const float du = un[c] * c_out + xv * c_skip;
     const float dc = cn[c] * c_out + xv * c_skip;
     const float den = du + sc * (dc - du);
-    const float d = (xv - den) / sigma;
-    float xn = xv + d * (sigma_next - sigma);
+    float xn;
+    if constexpr (kMultistep) {
+      const float4 k = coefs[step];
+      float dd = k.z * den;
+      if (k.w != 0.f) dd -= k.w * d_prev[idx];
+      xn = k.x * xv - k.y * dd;
+      d_prev[idx] = den;
+    } else {
+      const float d = (xv - den) / sigma;
+      xn = xv + d * (sigma_next - sigma);
+    }
     if (final_step && mask && cond_frame) xn = xn * (1.f - m) + cond_frame[idx] * m;
     x[idx] = xn;
   }
@@ -1224,8 +1237,24 @@ extern "C" int b200v_sampler_update(float* x, const float* net_out, int64_t ld_n
   VB_REQUIRE(x && net_out && scales && sigmas && step_idx, "sampler_update: null pointer");
   VB_REQUIRE(ld_net >= 4 && ld_net % 4 == 0, "sampler_update: ld_net must be a multiple of 4");
   const long long total = (long long)T * h * w;
-  sampler_update_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      x, net_out, cond_frame, mask, scales, sigmas, step_idx, num_steps, T, h, w, ld_net);
+  sampler_update_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      x, net_out, cond_frame, mask, scales, sigmas, step_idx, num_steps, T, h, w, ld_net, nullptr, nullptr);
+  step_inc_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_idx);
+  VB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b200v_sampler_update_2m(float* x, const float* net_out, int64_t ld_net, const float* cond_frame,
+                                       const float* mask, const float* scales, const float* coefs, float* d_prev,
+                                       const float* sigmas, int32_t* step_idx, int32_t num_steps, int32_t T, int32_t h,
+                                       int32_t w, void* stream) {
+  VB_REQUIRE(x && net_out && scales && coefs && d_prev && sigmas && step_idx, "sampler_update_2m: null pointer");
+  VB_REQUIRE(ld_net >= 4 && ld_net % 4 == 0, "sampler_update_2m: ld_net must be a multiple of 4");
+  VB_REQUIRE(((uintptr_t)coefs & 15) == 0, "sampler_update_2m: coefs must be 16-byte aligned");
+  const long long total = (long long)T * h * w;
+  sampler_update_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      x, net_out, cond_frame, mask, scales, sigmas, step_idx, num_steps, T, h, w, ld_net,
+      reinterpret_cast<const float4*>(coefs), d_prev);
   step_inc_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_idx);
   VB_CHECK_CUDA(cudaGetLastError());
   return 0;

@@ -8,6 +8,7 @@ Mirrors (paths relative to the reference root):
   Denoiser ................. vwm/modules/diffusionmodules/denoiser.py:10-35
   VanillaCFG / Identity / Linear / TrianglePredictionGuider ... guiders.py
   EulerEDMSampler .......... vwm/modules/diffusionmodules/sampling.py:15-124
+  DPMPP2MSampler ........... sgm's sampling.py DPMPP2MSampler (Vista does not ship it), on the same loop
   instantiate_from_config .. vwm/util.py:154-173
 
 The generic path keeps the reference's step algebra in torch (a dozen tiny fp32 ops per step on a
@@ -18,6 +19,7 @@ kernels per step around the UNet, no host synchronisation, no per-step tensor al
 from __future__ import annotations
 
 import importlib
+import math
 from typing import Dict, List, Optional, Union
 
 import torch
@@ -314,3 +316,57 @@ class EulerEDMSampler(BaseDiffusionSampler):
         return (isinstance(denoiser.network, B200Wrapper) and isinstance(denoiser.denoiser.scaling, VScalingWithEDMcNoise)
                 and isinstance(self.guider, (VanillaCFG, LinearPredictionGuider))
                 and all(k in cond for k in ("crossattn", "vector", "concat")))
+
+
+def dpmpp2m_coefficients(sigmas: torch.Tensor) -> torch.Tensor:
+    """(n, 4) float64 rows {a, b, c, e} of the DPM-Solver++(2M) step x = a x - b (c D - e D_prev) from the n + 1 sigmas
+    (Lu et al. 2022, arXiv 2211.01095, Algorithm 2; k-diffusion's sample_dpmpp_2m): with h_i = ln(s_i / s_i+1),
+    a = s_i+1 / s_i, b = expm1(-h_i); c = 1 + 1/(2 r), e = 1/(2 r), r = h_i-1 / h_i, except on the first step and on a
+    step to sigma = 0, which are first order (c = 1, e = 0; to sigma = 0 that is x = D).  Computed in double from the
+    sigma table the loop reads, so the fused kernel, its CPU twin and the torch loop apply the same coefficients."""
+    s = [float(v) for v in sigmas.detach().double().cpu()]
+    rows, h_prev = [], None
+    for i in range(len(s) - 1):
+        if s[i + 1] == 0.0:
+            rows.append((0.0, -1.0, 1.0, 0.0))
+            h_prev = None
+            continue
+        h = math.log(s[i] / s[i + 1])
+        if h_prev is None:
+            c, e = 1.0, 0.0
+        else:
+            e = h / (2.0 * h_prev)          # 1 / (2 r)
+            c = 1.0 + e
+        rows.append((s[i + 1] / s[i], math.expm1(-h), c, e))
+        h_prev = h
+    return torch.tensor(rows, dtype=torch.float64).reshape(-1, 4)
+
+
+class DPMPP2MSampler(BaseDiffusionSampler):
+    """DPM-Solver++(2M) (sgm's ``DPMPP2MSampler``): a second-order multistep solver of the sampling ODE at one network
+    evaluation per step, like Euler.  Same call as ``EulerEDMSampler``; the conditioning frames are re-imposed before
+    every step and after the loop (sampling.py:105-106,122-123), and the fused CUDA-graph loop runs under the same
+    conditions as Euler's."""
+
+    def __call__(self, denoiser, x, cond, uc=None, cond_frame=None, cond_mask=None, num_steps=None):
+        denoiser = _unwrap_reference_closure(denoiser)
+        if isinstance(denoiser, B200Denoiser) and self._fusable(denoiser, cond, uc):
+            from .fused import fused_sample
+            return fused_sample(self, denoiser, x, cond, uc, cond_frame, cond_mask, num_steps)
+        x, s_in, sigmas, num_sigmas, cond, uc = self.prepare_sampling_loop(x, cond, uc, num_steps)
+        coefs = dpmpp2m_coefficients(sigmas).tolist()
+        replace_cond_frames = cond_mask is not None and bool(cond_mask.any())
+        old_denoised = None
+        for i in self.get_sigma_gen(num_sigmas):
+            if replace_cond_frames:
+                x = x * append_dims(1 - cond_mask, x.ndim) + cond_frame * append_dims(cond_mask, cond_frame.ndim)
+            denoised = self.denoise(x, denoiser, s_in * sigmas[i], cond, cond_mask, uc)
+            a, b, c, e = coefs[i]
+            d = c * denoised if e == 0.0 else c * denoised - e * old_denoised
+            x = a * x - b * d
+            old_denoised = denoised
+        if replace_cond_frames:
+            x = x * append_dims(1 - cond_mask, x.ndim) + cond_frame * append_dims(cond_mask, cond_frame.ndim)
+        return x
+
+    _fusable = EulerEDMSampler._fusable

@@ -1,7 +1,8 @@
-"""Fused EDM/Euler sampling loop on the B200 executor.
+"""Fused EDM sampling loop on the B200 executor, for the Euler and the DPM-Solver++(2M) samplers.
 
 Per step: ``sampler_prepare`` (cond-frame re-imposition, c_in scaling, CFG batch doubling, concat,
-c_noise) -> UNet executor -> ``sampler_update`` (preconditioning, guidance, Euler step).  All state
+c_noise) -> UNet executor -> ``sampler_update`` (preconditioning, guidance, Euler step) or
+``sampler_update_2m`` (the same denoised value, then the 2M step from the host's coefficient table).  All state
 lives in persistent device buffers, the step index and sigma table are read on the device, so one
 step is a fixed launch sequence that is captured once in a CUDA graph and replayed (no host
 synchronisation inside the loop; the reference has two per step: sampling.py:102,109).
@@ -12,7 +13,7 @@ guiders.py:19-36,68-74; checked against the oracle in tests/test_sampler_gpu.py.
 from __future__ import annotations
 
 import os
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple
 
 import torch
 
@@ -44,7 +45,10 @@ class _LoopState:
         self.unet_in = padded_input_rows(2 * N * h * w, dev)
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.graph_steps = None
-        self.graphs: Dict[int, torch.cuda.CUDAGraph] = {}    # one captured step per schedule length (num_steps is a kernel argument)
+        # one captured step per (schedule length, 2M): num_steps is a kernel argument, and the two samplers' steps differ
+        self.graphs: Dict[Tuple[int, bool], torch.cuda.CUDAGraph] = {}
+        self.coefs: Optional[torch.Tensor] = None     # 2M only: [1024, 4] fp32 {a, b, c, e} per step
+        self.d_prev: Optional[torch.Tensor] = None    # 2M only: the previous step's denoised latent
         self.tape, self.tape_steps = None, None      # launch tape of one step (frame-sharded runtimes)
         # CFG-split mode (modules.enable_frame_sharding): this rank runs one half of the doubled batch
         self.split = None            # (half, pair process group)
@@ -97,7 +101,13 @@ class _LoopState:
         return rt.forward(self.unet_in[half * rows:(half + 1) * rows], self.c_noise[half * N:(half + 1) * N],
                           self.mask2[half * N:(half + 1) * N], h, w, net_out=out)
 
-    def _finish(self, net_out, num_steps: int):
+    def enable_multistep(self):
+        """Allocates the 2M sampler's coefficient table and D_prev buffer (once per state)."""
+        if self.d_prev is None:
+            self.coefs = torch.zeros(self.sigmas.numel(), 4, dtype=torch.float32, device=self.x.device)
+            self.d_prev = torch.empty_like(self.x)
+
+    def _finish(self, net_out, num_steps: int, multistep: bool = False):
         if self.split is not None and self.pair_peer is not None:
             # my half sits in net_full already (the output convolution wrote it there): store it into the partner's
             # net_full once the partner has consumed the previous step's (ack), raise its flag, wait for its half
@@ -111,25 +121,29 @@ class _LoopState:
             full, pg = self.net_full, self.split[1]
             _lib.tape_host(lambda src=net_out: dist.all_gather_into_tensor(full, src, group=pg), "cfg pair all_gather")   # bind now: net_out is rebound below
             net_out = full
-        ops.sampler_update(self.x, net_out, self.cond_frame, self.mask, self.scales, self.sigmas, self.step,
-                           num_steps, self.N, self.h, self.w)
+        if multistep:
+            ops.sampler_update_2m(self.x, net_out, self.cond_frame, self.mask, self.scales, self.coefs, self.d_prev,
+                                  self.sigmas, self.step, num_steps, self.N, self.h, self.w)
+        else:
+            ops.sampler_update(self.x, net_out, self.cond_frame, self.mask, self.scales, self.sigmas, self.step,
+                               num_steps, self.N, self.h, self.w)
         if self.split is not None and self.pair_peer is not None:      # the partner may overwrite my copy of its half now
             pp = self.pair_peer
             ops.peer_put(pp["ack_src"], 16, 1, 16, pp["ack_dst"], 16, pp["ack_flag_remote"], 1, pp["c_ack_put"], pp["t_ack"], "cfg ack")
 
-    def one_step(self, rt, num_steps: int):
+    def one_step(self, rt, num_steps: int, multistep: bool = False):
         self._prepare()
-        self._finish(self._forward(rt), num_steps)
+        self._finish(self._forward(rt), num_steps, multistep)
 
-    def runner(self, rt, num_steps: int):
+    def runner(self, rt, num_steps: int, multistep: bool = False):
         """Callable advancing one step the fastest supported way; call after one eager step (which allocates every
         buffer of the executor).  Without a collective inside the UNet the launch sequence is replayed from a CUDA
         graph: the whole step, or prepare + UNet in CFG-split mode (the pair exchange and the update stay eager)."""
         if not USE_GRAPH:
-            return lambda: self.one_step(rt, num_steps)
+            return lambda: self.one_step(rt, num_steps, multistep)
         # NB: `rt.group is None` also names the DEFAULT process group; the runtime says whether its step holds collectives
         if getattr(rt, "has_collectives", False) and not USE_TAPE:
-            return lambda: self.one_step(rt, num_steps)
+            return lambda: self.one_step(rt, num_steps, multistep)
         if getattr(rt, "has_collectives", False):
             # collectives inside the UNet: no graph; the first call records the step's C-ABI calls and host-side
             # collectives on a launch tape (vista_b200.lib), later calls replay it without the Python layers above
@@ -144,20 +158,21 @@ class _LoopState:
                 else:
                     _lib.replay(self.tape)
             return run_taped
-        if num_steps in self.graphs:
-            self.graph, self.graph_steps = self.graphs[num_steps], num_steps
-        if self.graph is None or self.graph_steps != num_steps:
+        key = (num_steps, multistep)
+        if key in self.graphs:
+            self.graph, self.graph_steps = self.graphs[key], key
+        if self.graph is None or self.graph_steps != key:
             g = torch.cuda.CUDAGraph()
             torch.cuda.synchronize()
             whole = self.split is None or self.pair_peer is not None      # no host-side collective in the step
             with torch.cuda.graph(g):             # capture does not execute
                 if whole:
-                    self.one_step(rt, num_steps)
+                    self.one_step(rt, num_steps, multistep)
                 else:
                     self._prepare()
                     self._fwd_out = self._forward(rt)
-            self.graph, self.graph_steps = g, num_steps
-            self.graphs[num_steps] = g
+            self.graph, self.graph_steps = g, key
+            self.graphs[key] = g
         if self.split is None or self.pair_peer is not None:
             return self.graph.replay
 
@@ -183,6 +198,10 @@ def fused_sample(sampler, den, x: torch.Tensor, cond: Dict, uc: Optional[Dict], 
     dev = x.device
     N, zc, h, w = x.shape
     assert zc == 4 and N % T == 0
+    from .diffusion import DPMPP2MSampler, dpmpp2m_coefficients
+    multistep = isinstance(sampler, DPMPP2MSampler)
+    if multistep and getattr(net, "frame_sharded", False):
+        raise NotImplementedError("DPMPP2MSampler: the frame-sharded fused loop runs the Euler sampler only")
     rt = net._rt_get(net.diffusion_model, T, dev)
     if getattr(net, "frame_sharded", False):
         return _fused_sample_sharded(sampler, rt, x, cond, uc, cond_frame, cond_mask, n, T, net)
@@ -197,6 +216,9 @@ def fused_sample(sampler, den, x: torch.Tensor, cond: Dict, uc: Optional[Dict], 
     x *= torch.sqrt(1.0 + sigmas[0] ** 2).to(x.device)            # sampling.py:36 (in place, like the reference)
     st.x.copy_(x)
     st.sigmas[: n + 1].copy_(sigmas)
+    if multistep:
+        st.enable_multistep()
+        st.coefs[:n].copy_(dpmpp2m_coefficients(sigmas).to(torch.float32))
     st.step.zero_()
     if cond_frame is not None:
         st.cond_frame.copy_(cond_frame)
@@ -213,18 +235,18 @@ def fused_sample(sampler, den, x: torch.Tensor, cond: Dict, uc: Optional[Dict], 
     y = torch.cat((_expand(uc["vector"], N, T), _expand(cond["vector"], N, T)), 0)
     rt.set_conditioning(context, y)
 
-    _run_steps(st, rt, n)
+    _run_steps(st, rt, n, multistep)
     x.copy_(st.x)
     return x
 
 
-def _run_steps(st: _LoopState, rt, n: int):
+def _run_steps(st: _LoopState, rt, n: int, multistep: bool = False):
     if n < 3:
         for _ in range(n):
-            st.one_step(rt, n)
+            st.one_step(rt, n, multistep)
         return
-    st.one_step(rt, n)                          # eager first step: allocates every buffer of the executor
-    step = st.runner(rt, n)
+    st.one_step(rt, n, multistep)               # eager first step: allocates every buffer of the executor
+    step = st.runner(rt, n, multistep)
     for _ in range(n - 1):
         step()
 

@@ -548,6 +548,18 @@ def sampler_update(x, net_out, cond_frame, mask, scales, sigmas, step_idx, num_s
     _prof_end()
 
 
+def sampler_update_2m(x, net_out, cond_frame, mask, scales, coefs, d_prev, sigmas, step_idx, num_steps, T, h, w):
+    """The DPM-Solver++(2M) step: ``coefs`` is the fp32 (>= num_steps, 4) table of ``diffusion.dpmpp2m_coefficients``,
+    ``d_prev`` the (T, 4, h, w) fp32 denoised value of the previous step (read only on second-order rows)."""
+    _count(2)
+    _prof_begin("other", "sampler_update_2m", 0.0, 0.0)
+    _lib.check(_lib.load().b200v_sampler_update_2m(x.data_ptr(), net_out.data_ptr(), net_out.stride(0), _ptr(cond_frame),
+                                                   _ptr(mask), scales.data_ptr(), coefs.data_ptr(), d_prev.data_ptr(),
+                                                   sigmas.data_ptr(), step_idx.data_ptr(), num_steps, T, h, w, _stream()),
+               "b200v_sampler_update_2m")
+    _prof_end()
+
+
 def nchw_to_tokens(x, out, NB, Cc, H, W):
     _count(1)
     _prof_begin("other", "nchw_to_tokens", 0.0, 0.0)
