@@ -218,6 +218,10 @@ int b200v_blend_emb(const float* e_plain, const float* e_cond, const float* labe
  *            c = 1 + 1/(2r), e = 1/(2r), r = h_prev/h; c = 1, e = 0 on a first-order row):
  *            x = a*x - b*(c*D - e*d_prev); d_prev = D             (d_prev is not read when e == 0)
  *            and, when `final`, re-imposes the conditioning frames
+ *   update_action: action guidance (vista_b200.diffusion.ActionCFG, InstructPix2Pix eq. 3): D_img = the denoised value of
+ *            row t of net_img (the conditional rows with the action slots of crossattn zeroed),
+ *            D = D_u + scales[t]*(D_img - D_u) + action_scales[t]*(D_c - D_img); then the Euler step
+ *            (coefs == d_prev == NULL) or the 2M step (both given), as in update / update_2m
  * ---------------------------------------------------------------------------------------------- */
 int b200v_sampler_prepare(float* x, const float* cond_frame, const float* mask,
                           const float* concat_u /* uncond rows (T,4,h,w) or NULL = zeros */,
@@ -232,6 +236,13 @@ int b200v_sampler_update_2m(float* x, const float* net_out /* as in b200v_sample
                             const float* coefs /* [num_steps, 4] fp32 {a, b, c, e}, 16-byte aligned */,
                             float* d_prev /* (T,4,h,w) fp32, the previous step's D */, const float* sigmas,
                             int32_t* step_idx, int32_t num_steps, int32_t T, int32_t h, int32_t w, void* stream);
+int b200v_sampler_update_action(float* x, const float* net_out /* as in b200v_sampler_update */, int64_t ld_net,
+                                const float* net_img /* [T*h*w, ld_img] fp32 token-major, 4 channels used */,
+                                int64_t ld_img, const float* cond_frame, const float* mask,
+                                const float* scales /* [T] s_img */, const float* action_scales /* [T] s_act */,
+                                const float* coefs /* as in update_2m, or NULL */, float* d_prev /* or NULL */,
+                                const float* sigmas, int32_t* step_idx, int32_t num_steps, int32_t T, int32_t h,
+                                int32_t w, void* stream);
 
 /* VAE decoder helpers.
  *   softmax_rows : fp32 scores -> fp16 probabilities, one row per block (mid.attn_1 single-head d=512

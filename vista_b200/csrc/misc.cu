@@ -803,15 +803,20 @@ __global__ void sampler_prepare_kernel(float* __restrict__ x, const float* __res
   *reinterpret_cast<uint4*>(unet_in + (((long long)T + t) * hw + pix) * ld_in) = f_to_h8(cu);
 }
 
-// <false>: the Euler step.  <true>: the DPM-Solver++(2M) step x = a x - b (c D - e D_prev), D_prev = D, with
+// kMultistep <false>: the Euler step.  <true>: the DPM-Solver++(2M) step x = a x - b (c D - e D_prev), D_prev = D, with
 // {a, b, c, e} = coefs[step] from the host (vista_b200.diffusion.dpmpp2m_coefficients); e == 0 marks a first-order
 // row, on which D_prev is not read (it is uninitialised at a sample's first step).
-template <bool kMultistep>
+// kActionCfg <true>: action guidance (vista_b200.diffusion.ActionCFG).  D_img, the denoised value of the conditional rows
+// with the action slots zeroed, is row t of net_img; D = D_u + s_img (D_img - D_u) + s_act (D_c - D_img), in the torch
+// guider's order, with s_img = scales[t] and s_act = action_scales[t] read on the device (a captured graph replays them).
+template <bool kMultistep, bool kActionCfg>
 __global__ void sampler_update_kernel(float* __restrict__ x, const float* __restrict__ net,
                                       const float* __restrict__ cond_frame, const float* __restrict__ mask,
                                       const float* __restrict__ scales, const float* __restrict__ sigmas,
                                       const int* __restrict__ step_idx, int num_steps, int T, int h, int w,
-                                      long long ld_net, const float4* __restrict__ coefs, float* __restrict__ d_prev) {
+                                      long long ld_net, const float4* __restrict__ coefs, float* __restrict__ d_prev,
+                                      const float* __restrict__ net_img, long long ld_img,
+                                      const float* __restrict__ action_scales) {
   const int step = *step_idx;
   const float sigma = sigmas[step], sigma_next = sigmas[step + 1];
   const float c_skip = 1.0f / (sigma * sigma + 1.0f);
@@ -825,6 +830,12 @@ __global__ void sampler_update_kernel(float* __restrict__ x, const float* __rest
   const float4 nc = *reinterpret_cast<const float4*>(net + (((long long)T + t) * hw + pix) * ld_net);
   const float un[4] = {nu.x, nu.y, nu.z, nu.w}, cn[4] = {nc.x, nc.y, nc.z, nc.w};
   const float sc = scales[t];
+  float in[4] = {0.f, 0.f, 0.f, 0.f}, sa = 0.f;
+  if constexpr (kActionCfg) {
+    const float4 ni = *reinterpret_cast<const float4*>(net_img + ((long long)t * hw + pix) * ld_img);
+    in[0] = ni.x; in[1] = ni.y; in[2] = ni.z; in[3] = ni.w;
+    sa = action_scales[t];
+  }
   const bool final_step = (step + 1 == num_steps);
   const float m = mask ? mask[t] : 0.f;
 #pragma unroll
@@ -833,7 +844,14 @@ __global__ void sampler_update_kernel(float* __restrict__ x, const float* __rest
     const float xv = x[idx];
     const float du = un[c] * c_out + xv * c_skip;
     const float dc = cn[c] * c_out + xv * c_skip;
-    const float den = du + sc * (dc - du);
+    float den;
+    if constexpr (kActionCfg) {
+      const float di = in[c] * c_out + xv * c_skip;
+      den = du + sc * (di - du);
+      den = den + sa * (dc - di);
+    } else {
+      den = du + sc * (dc - du);
+    }
     float xn;
     if constexpr (kMultistep) {
       const float4 k = coefs[step];
@@ -1237,8 +1255,9 @@ extern "C" int b200v_sampler_update(float* x, const float* net_out, int64_t ld_n
   VB_REQUIRE(x && net_out && scales && sigmas && step_idx, "sampler_update: null pointer");
   VB_REQUIRE(ld_net >= 4 && ld_net % 4 == 0, "sampler_update: ld_net must be a multiple of 4");
   const long long total = (long long)T * h * w;
-  sampler_update_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      x, net_out, cond_frame, mask, scales, sigmas, step_idx, num_steps, T, h, w, ld_net, nullptr, nullptr);
+  sampler_update_kernel<false, false><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      x, net_out, cond_frame, mask, scales, sigmas, step_idx, num_steps, T, h, w, ld_net, nullptr, nullptr, nullptr, 0,
+      nullptr);
   step_inc_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_idx);
   VB_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -1252,9 +1271,36 @@ extern "C" int b200v_sampler_update_2m(float* x, const float* net_out, int64_t l
   VB_REQUIRE(ld_net >= 4 && ld_net % 4 == 0, "sampler_update_2m: ld_net must be a multiple of 4");
   VB_REQUIRE(((uintptr_t)coefs & 15) == 0, "sampler_update_2m: coefs must be 16-byte aligned");
   const long long total = (long long)T * h * w;
-  sampler_update_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+  sampler_update_kernel<true, false><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       x, net_out, cond_frame, mask, scales, sigmas, step_idx, num_steps, T, h, w, ld_net,
-      reinterpret_cast<const float4*>(coefs), d_prev);
+      reinterpret_cast<const float4*>(coefs), d_prev, nullptr, 0, nullptr);
+  step_inc_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_idx);
+  VB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b200v_sampler_update_action(float* x, const float* net_out, int64_t ld_net, const float* net_img,
+                                           int64_t ld_img, const float* cond_frame, const float* mask, const float* scales,
+                                           const float* action_scales, const float* coefs, float* d_prev,
+                                           const float* sigmas, int32_t* step_idx, int32_t num_steps, int32_t T,
+                                           int32_t h, int32_t w, void* stream) {
+  VB_REQUIRE(x && net_out && net_img && scales && action_scales && sigmas && step_idx,
+             "sampler_update_action: null pointer");
+  VB_REQUIRE(ld_net >= 4 && ld_net % 4 == 0, "sampler_update_action: ld_net must be a multiple of 4");
+  VB_REQUIRE(ld_img >= 4 && ld_img % 4 == 0, "sampler_update_action: ld_img must be a multiple of 4");
+  VB_REQUIRE((coefs == nullptr) == (d_prev == nullptr),
+             "sampler_update_action: coefs and d_prev are both NULL (Euler) or both given (2M)");
+  VB_REQUIRE(((uintptr_t)coefs & 15) == 0, "sampler_update_action: coefs must be 16-byte aligned");
+  const long long total = (long long)T * h * w;
+  const unsigned grid = (unsigned)((total + 255) / 256);
+  if (coefs)
+    sampler_update_kernel<true, true><<<grid, 256, 0, (cudaStream_t)stream>>>(
+        x, net_out, cond_frame, mask, scales, sigmas, step_idx, num_steps, T, h, w, ld_net,
+        reinterpret_cast<const float4*>(coefs), d_prev, net_img, ld_img, action_scales);
+  else
+    sampler_update_kernel<false, true><<<grid, 256, 0, (cudaStream_t)stream>>>(
+        x, net_out, cond_frame, mask, scales, sigmas, step_idx, num_steps, T, h, w, ld_net, nullptr, nullptr, net_img,
+        ld_img, action_scales);
   step_inc_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_idx);
   VB_CHECK_CUDA(cudaGetLastError());
   return 0;

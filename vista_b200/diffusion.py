@@ -7,6 +7,7 @@ Mirrors (paths relative to the reference root):
   VScalingWithEDMcNoise & co vwm/modules/diffusionmodules/denoiser_scaling.py
   Denoiser ................. vwm/modules/diffusionmodules/denoiser.py:10-35
   VanillaCFG / Identity / Linear / TrianglePredictionGuider ... guiders.py
+  ActionCFG ................ a separate guidance scale for the action (not in Vista; InstructPix2Pix's two-scale CFG)
   EulerEDMSampler .......... vwm/modules/diffusionmodules/sampling.py:15-124
   DPMPP2MSampler ........... sgm's sampling.py DPMPP2MSampler (Vista does not ship it), on the same loop
   instantiate_from_config .. vwm/util.py:154-173
@@ -212,6 +213,61 @@ class TrianglePredictionGuider(LinearPredictionGuider):
         return 2 * (values / period - torch.floor(values / period + 0.5)).abs()
 
 
+class ActionCFG(Guider):
+    """Classifier-free guidance with a separate scale for the driving action (Brooks et al. 2023, InstructPix2Pix,
+    arXiv 2211.09800, eq. 3; Liu et al. 2022, Composable Diffusion):
+
+        D = D_u + s_img (D_img - D_u) + s_act (D_c - D_img)
+
+    D_u and D_c are the denoiser on ``uc`` and ``c``; D_img is the denoiser on ``c`` with every action slot zeroed
+    (``action_free``), which Vista's action training puts in distribution (each action embedder is dropped on its own,
+    ucg_rate 0.15).  ``guider_config`` is the image guider (VanillaCFG, Linear- or TrianglePredictionGuider): it gives
+    the per-frame s_img and applies the image term; ``action_scale`` is s_act for every frame.  With s_act == s_img this
+    is the image guider alone; with no action in ``c``, D_c == D_img.  One more network evaluation per step on the
+    conditional rows."""
+
+    def __init__(self, action_scale: float, guider_config: Dict, context_dim: int = 1024):
+        self.action_scale = float(action_scale)
+        self.image_guider = instantiate_from_config(guider_config)
+        self.context_dim = context_dim
+        self.additional_cond_keys = list(self.image_guider.additional_cond_keys)
+
+    def action_free(self, c: Dict) -> Dict:
+        """``c`` with its action slots zeroed: every action key is a crossattn slot in the columns after the CLIP
+        embedding's ``context_dim``, and a zeroed or missing action key is a zero slot (encoders/modules.py:128-130).
+        The other keys are shared, not copied."""
+        out = dict(c)
+        ctx = c["crossattn"].clone()
+        ctx[..., self.context_dim:] = 0.0
+        out["crossattn"] = ctx
+        return out
+
+    def __call__(self, x, sigma):
+        x_u, x_img, x_c = x.chunk(3)
+        return self.image_guider(torch.cat((x_u, x_img)), sigma) + self.action_scale * (x_c - x_img)
+
+    def prepare_inputs(self, x, s, c, cond_mask, uc):
+        """Three batches (uc, action-free c, c): crossattn from those three, every other merged key from (uc, c, c)."""
+        c_img = self.action_free(c)
+        c_out = dict()
+        for k in c:
+            if k == "crossattn":
+                c_out[k] = torch.cat((uc[k], c_img[k], c[k]), 0)
+            elif k in ["vector", "concat"] + list(self.additional_cond_keys):
+                c_out[k] = torch.cat((uc[k], c[k], c[k]), 0)
+            else:
+                assert c[k] == uc[k]
+                c_out[k] = c[k]
+        return torch.cat([x] * 3), torch.cat([s] * 3), c_out, torch.cat([cond_mask] * 3)
+
+    def scale_vector(self, num_frames):
+        return self.image_guider.scale_vector(num_frames)
+
+    def action_scale_vector(self, num_frames):
+        """Per-frame s_act (fused path): ``action_scale`` on every frame."""
+        return torch.full((num_frames,), self.action_scale)
+
+
 # ----------------------------------------------------------------------------------------------
 # sampler
 # ----------------------------------------------------------------------------------------------
@@ -313,8 +369,9 @@ class EulerEDMSampler(BaseDiffusionSampler):
 
     def _fusable(self, denoiser: "B200Denoiser", cond, uc) -> bool:
         from .modules import B200Wrapper
+        guider = self.guider.image_guider if isinstance(self.guider, ActionCFG) else self.guider
         return (isinstance(denoiser.network, B200Wrapper) and isinstance(denoiser.denoiser.scaling, VScalingWithEDMcNoise)
-                and isinstance(self.guider, (VanillaCFG, LinearPredictionGuider))
+                and isinstance(guider, (VanillaCFG, LinearPredictionGuider))
                 and all(k in cond for k in ("crossattn", "vector", "concat")))
 
 

@@ -2,7 +2,9 @@
 
 Per step: ``sampler_prepare`` (cond-frame re-imposition, c_in scaling, CFG batch doubling, concat,
 c_noise) -> UNet executor -> ``sampler_update`` (preconditioning, guidance, Euler step) or
-``sampler_update_2m`` (the same denoised value, then the 2M step from the host's coefficient table).  All state
+``sampler_update_2m`` (the same denoised value, then the 2M step from the host's coefficient table).  Under action
+guidance (``diffusion.ActionCFG``) a second, T-row forward runs the conditional half of the prepared batch under the
+action-free conditioning, and ``sampler_update_action`` combines the three denoised values.  All state
 lives in persistent device buffers, the step index and sigma table are read on the device, so one
 step is a fixed launch sequence that is captured once in a CUDA graph and replayed (no host
 synchronisation inside the loop; the reference has two per step: sampling.py:102,109).
@@ -45,10 +47,16 @@ class _LoopState:
         self.unet_in = padded_input_rows(2 * N * h * w, dev)
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.graph_steps = None
-        # one captured step per (schedule length, 2M): num_steps is a kernel argument, and the two samplers' steps differ
-        self.graphs: Dict[Tuple[int, bool], torch.cuda.CUDAGraph] = {}
+        # one captured step per (schedule length, 2M), and per (schedule length, 2M, True) under action guidance:
+        # num_steps is a kernel argument, and the steps differ
+        self.graphs: Dict[Tuple, torch.cuda.CUDAGraph] = {}
         self.coefs: Optional[torch.Tensor] = None     # 2M only: [1024, 4] fp32 {a, b, c, e} per step
         self.d_prev: Optional[torch.Tensor] = None    # 2M only: the previous step's denoised latent
+        # action guidance only: per-frame s_act on the device (a captured graph replays the values set per sample), the
+        # action-free conditioning of the conditional rows, and the output of the T-row forward that reads it
+        self.action_scales: Optional[torch.Tensor] = None
+        self.img_cond = None          # (crossattn, vector) of the N image rows, as last handed to the runtime
+        self.net_img: Optional[torch.Tensor] = None
         self.tape, self.tape_steps = None, None      # launch tape of one step (frame-sharded runtimes)
         # CFG-split mode (modules.enable_frame_sharding): this rank runs one half of the doubled batch
         self.split = None            # (half, pair process group)
@@ -101,13 +109,25 @@ class _LoopState:
         return rt.forward(self.unet_in[half * rows:(half + 1) * rows], self.c_noise[half * N:(half + 1) * N],
                           self.mask2[half * N:(half + 1) * N], h, w, net_out=out)
 
+    def _forward_img(self, rt):
+        """The action-free image branch: the conditional half of the prepared batch (rows bit for bit what the branch
+        needs) through an N-row forward under the runtime's N-row conditioning."""
+        N, h, w = self.N, self.h, self.w
+        self.net_img = rt.forward(self.unet_in[N * h * w:], self.c_noise[N:], self.mask2[N:], h, w)
+        return self.net_img
+
+    def enable_action(self):
+        """Allocates the per-frame action scale (once per state)."""
+        if self.action_scales is None:
+            self.action_scales = torch.zeros_like(self.scales)
+
     def enable_multistep(self):
         """Allocates the 2M sampler's coefficient table and D_prev buffer (once per state)."""
         if self.d_prev is None:
             self.coefs = torch.zeros(self.sigmas.numel(), 4, dtype=torch.float32, device=self.x.device)
             self.d_prev = torch.empty_like(self.x)
 
-    def _finish(self, net_out, num_steps: int, multistep: bool = False):
+    def _finish(self, net_out, num_steps: int, multistep: bool = False, net_img=None):
         if self.split is not None and self.pair_peer is not None:
             # my half sits in net_full already (the output convolution wrote it there): store it into the partner's
             # net_full once the partner has consumed the previous step's (ack), raise its flag, wait for its half
@@ -121,7 +141,11 @@ class _LoopState:
             full, pg = self.net_full, self.split[1]
             _lib.tape_host(lambda src=net_out: dist.all_gather_into_tensor(full, src, group=pg), "cfg pair all_gather")   # bind now: net_out is rebound below
             net_out = full
-        if multistep:
+        if net_img is not None:
+            ops.sampler_update_action(self.x, net_out, net_img, self.cond_frame, self.mask, self.scales, self.action_scales,
+                                      self.coefs if multistep else None, self.d_prev if multistep else None, self.sigmas,
+                                      self.step, num_steps, self.N, self.h, self.w)
+        elif multistep:
             ops.sampler_update_2m(self.x, net_out, self.cond_frame, self.mask, self.scales, self.coefs, self.d_prev,
                                   self.sigmas, self.step, num_steps, self.N, self.h, self.w)
         else:
@@ -131,19 +155,20 @@ class _LoopState:
             pp = self.pair_peer
             ops.peer_put(pp["ack_src"], 16, 1, 16, pp["ack_dst"], 16, pp["ack_flag_remote"], 1, pp["c_ack_put"], pp["t_ack"], "cfg ack")
 
-    def one_step(self, rt, num_steps: int, multistep: bool = False):
+    def one_step(self, rt, num_steps: int, multistep: bool = False, action: bool = False):
         self._prepare()
-        self._finish(self._forward(rt), num_steps, multistep)
+        net_out = self._forward(rt)
+        self._finish(net_out, num_steps, multistep, self._forward_img(rt) if action else None)
 
-    def runner(self, rt, num_steps: int, multistep: bool = False):
+    def runner(self, rt, num_steps: int, multistep: bool = False, action: bool = False):
         """Callable advancing one step the fastest supported way; call after one eager step (which allocates every
         buffer of the executor).  Without a collective inside the UNet the launch sequence is replayed from a CUDA
         graph: the whole step, or prepare + UNet in CFG-split mode (the pair exchange and the update stay eager)."""
         if not USE_GRAPH:
-            return lambda: self.one_step(rt, num_steps, multistep)
+            return lambda: self.one_step(rt, num_steps, multistep, action)
         # NB: `rt.group is None` also names the DEFAULT process group; the runtime says whether its step holds collectives
         if getattr(rt, "has_collectives", False) and not USE_TAPE:
-            return lambda: self.one_step(rt, num_steps, multistep)
+            return lambda: self.one_step(rt, num_steps, multistep, action)
         if getattr(rt, "has_collectives", False):
             # collectives inside the UNet: no graph; the first call records the step's C-ABI calls and host-side
             # collectives on a launch tape (vista_b200.lib), later calls replay it without the Python layers above
@@ -158,7 +183,7 @@ class _LoopState:
                 else:
                     _lib.replay(self.tape)
             return run_taped
-        key = (num_steps, multistep)
+        key = (num_steps, multistep, True) if action else (num_steps, multistep)
         if key in self.graphs:
             self.graph, self.graph_steps = self.graphs[key], key
         if self.graph is None or self.graph_steps != key:
@@ -167,7 +192,7 @@ class _LoopState:
             whole = self.split is None or self.pair_peer is not None      # no host-side collective in the step
             with torch.cuda.graph(g):             # capture does not execute
                 if whole:
-                    self.one_step(rt, num_steps, multistep)
+                    self.one_step(rt, num_steps, multistep, action)
                 else:
                     self._prepare()
                     self._fwd_out = self._forward(rt)
@@ -198,10 +223,13 @@ def fused_sample(sampler, den, x: torch.Tensor, cond: Dict, uc: Optional[Dict], 
     dev = x.device
     N, zc, h, w = x.shape
     assert zc == 4 and N % T == 0
-    from .diffusion import DPMPP2MSampler, dpmpp2m_coefficients
+    from .diffusion import ActionCFG, DPMPP2MSampler, dpmpp2m_coefficients
     multistep = isinstance(sampler, DPMPP2MSampler)
+    action = isinstance(sampler.guider, ActionCFG)
     if multistep and getattr(net, "frame_sharded", False):
         raise NotImplementedError("DPMPP2MSampler: the frame-sharded fused loop runs the Euler sampler only")
+    if action and getattr(net, "frame_sharded", False):
+        raise NotImplementedError("ActionCFG: the frame-sharded fused loop runs one guidance scale only")
     rt = net._rt_get(net.diffusion_model, T, dev)
     if getattr(net, "frame_sharded", False):
         return _fused_sample_sharded(sampler, rt, x, cond, uc, cond_frame, cond_mask, n, T, net)
@@ -234,19 +262,24 @@ def fused_sample(sampler, den, x: torch.Tensor, cond: Dict, uc: Optional[Dict], 
     context = torch.cat((_expand(uc["crossattn"], N, T), _expand(cond["crossattn"], N, T)), 0)
     y = torch.cat((_expand(uc["vector"], N, T), _expand(cond["vector"], N, T)), 0)
     rt.set_conditioning(context, y)
+    if action:
+        st.enable_action()
+        st.action_scales.copy_(sampler.guider.action_scale_vector(T).to(dev, torch.float32).repeat(N // T))
+        st.img_cond = (_expand(sampler.guider.action_free(cond)["crossattn"], N, T), y[N:])
+        rt.set_conditioning(*st.img_cond)
 
-    _run_steps(st, rt, n, multistep)
+    _run_steps(st, rt, n, multistep, action)
     x.copy_(st.x)
     return x
 
 
-def _run_steps(st: _LoopState, rt, n: int, multistep: bool = False):
+def _run_steps(st: _LoopState, rt, n: int, multistep: bool = False, action: bool = False):
     if n < 3:
         for _ in range(n):
-            st.one_step(rt, n, multistep)
+            st.one_step(rt, n, multistep, action)
         return
-    st.one_step(rt, n, multistep)               # eager first step: allocates every buffer of the executor
-    step = st.runner(rt, n, multistep)
+    st.one_step(rt, n, multistep, action)       # eager first step: allocates every buffer of the executor
+    step = st.runner(rt, n, multistep, action)
     for _ in range(n - 1):
         step()
 

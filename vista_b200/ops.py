@@ -560,6 +560,22 @@ def sampler_update_2m(x, net_out, cond_frame, mask, scales, coefs, d_prev, sigma
     _prof_end()
 
 
+def sampler_update_action(x, net_out, net_img, cond_frame, mask, scales, action_scales, coefs, d_prev, sigmas, step_idx,
+                          num_steps, T, h, w):
+    """The step under action guidance: ``net_img`` is the [T h w, >= 4] fp32 output of the conditional rows with the
+    action slots zeroed, ``action_scales`` the (T,) device array of s_act.  ``coefs`` / ``d_prev`` as in
+    ``sampler_update_2m`` for the 2M step, both None for the Euler step."""
+    _count(2)
+    _prof_begin("other", "sampler_update_action", 0.0, 0.0)
+    _lib.check(_lib.load().b200v_sampler_update_action(x.data_ptr(), net_out.data_ptr(), net_out.stride(0),
+                                                       net_img.data_ptr(), net_img.stride(0), _ptr(cond_frame), _ptr(mask),
+                                                       scales.data_ptr(), action_scales.data_ptr(), _ptr(coefs),
+                                                       _ptr(d_prev), sigmas.data_ptr(), step_idx.data_ptr(), num_steps, T,
+                                                       h, w, _stream()),
+               "b200v_sampler_update_action")
+    _prof_end()
+
+
 def nchw_to_tokens(x, out, NB, Cc, H, W):
     _count(1)
     _prof_begin("other", "nchw_to_tokens", 0.0, 0.0)

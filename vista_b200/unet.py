@@ -58,6 +58,7 @@ class UNetRuntime:
         self._pack()
         self._sd = None
         self.cond = None
+        self.conds: Dict[int, dict] = {}      # batch size -> its conditioning; forward(B rows) uses conds[B]
 
     # ------------------------------------------------------------------ weight packing
     def _f32(self, name):
@@ -225,7 +226,9 @@ class UNetRuntime:
         return out
 
     def set_conditioning(self, context: torch.Tensor, y: torch.Tensor):
-        """context (B,1,3456) / y (B,768): everything that does not depend on sigma or the step."""
+        """context (B,1,3456) / y (B,768): everything that does not depend on sigma or the step.  One conditioning is
+        kept per batch size B (its constants are buffers of B rows), so that the CFG pair's 2T rows and action guidance's
+        T image rows are conditioned side by side; setting B again replaces only B's."""
         T = self.T
         B = context.shape[0]
         # both cross-attentions are folded to per-frame constants, which is exact for ONE key token only
@@ -249,7 +252,7 @@ class UNetRuntime:
             temb = self.buf("cond.temb", T, t.ch)
             ops.timestep_embedding(frames, temb, t.ch)
             cond["pos"][t.prefix] = self._mlp(temb, *L["pos"], f"cond.pos.{t.prefix}")
-        self.cond = cond
+        self.cond = self.conds[B] = cond
 
     # ------------------------------------------------------------------ layers
     def _fuse_stats(self, B, h, w) -> bool:
@@ -346,10 +349,11 @@ class UNetRuntime:
         """x_tokens: [(B h w), 8] fp16 (x*c_in | concat), either contiguous or a view of zero-padded IN_PAD-wide rows
         (padded_input_rows); c_noise: [B] fp32; returns [(B h w), 8] fp32 whose first out_channels columns are the
         network output."""
-        assert self.cond is not None, "call set_conditioning() first"
         cfg, T = self.cfg, self.T
         B = c_noise.numel()
-        assert B % T == 0 and x_tokens.shape[0] == B * h * w and self.cond["B"] == B
+        assert B in self.conds, f"call set_conditioning() with {B} rows first"
+        self.cond = self.conds[B]
+        assert B % T == 0 and x_tokens.shape[0] == B * h * w
         mc, ed = cfg.model_channels, cfg.time_embed_dim
         # GroupNorm statistics / scratch are persistent per batch size (never replaced or freed): CUDA graphs and launch
         # tapes captured for another (B, h, w) keep replaying against the buffers they were captured with
