@@ -108,6 +108,9 @@ def groupnorm(x, y, frames, tokens_per_frame, gamma, beta, eps, silu, stats=None
     xs = _f(x[:, :C]).reshape(frames // frames_per_stat, frames_per_stat * tokens_per_frame, groups, C // groups)
     mean = xs.mean(dim=(1, 3), keepdim=True)
     var = xs.var(dim=(1, 3), unbiased=False, keepdim=True)
+    if stats is not None:                        # the kernel's (mean, rstd) output
+        stats[..., 0] = mean.reshape(stats.shape[:2])
+        stats[..., 1] = torch.rsqrt(var + eps).reshape(stats.shape[:2])
     o = ((xs - mean) * torch.rsqrt(var + eps)).reshape(-1, C) * _f(gamma) + _f(beta)
     if silu:
         o = F.silu(o)

@@ -235,30 +235,35 @@ def make_gemm_case(c, device):
     return dict(a=a, w=w, out=out, obuf=obuf, kw=kw, M=M, N=N, K=K, cin=cin, n_out=n_out)
 
 
-def im2col64(a, cin, taps, geom, h_pad, rows=None):
+def im2col64(a, cin, taps, geom, h_pad, rows=None, upsample=False):
     """fp64 implicit-GEMM operand [tokens (or `rows`), ntaps * cin]: out row (b, h, w) reads a[b, h + h_pad + dh, w + dw],
-    zero outside the stored rows (the halo slots are real rows)."""
+    zero outside the stored rows (the halo slots are real rows).  ``upsample``: the taps run over the nearest-2x
+    upsampled view of ``a`` (geometry ``geom``): out row (b, y, x) of the 2H x 2W frame reads a[b, (y + dh) // 2,
+    (x + dw) // 2], zero outside the upsampled frame."""
     if geom is None:
         x = a[:, :cin] if rows is None else a[rows, :cin]
         return x.double()
     W, H, NB = geom
+    s = 2 if upsample else 1
     He = H + 2 * h_pad
-    tok = torch.arange(W * H * NB, device=a.device) if rows is None else rows
-    w, h, b = tok % W, (tok // W) % H, tok // (W * H)
+    tok = torch.arange(W * H * NB * s * s, device=a.device) if rows is None else rows
+    w, h, b = tok % (s * W), (tok // (s * W)) % (s * H), tok // (s * s * W * H)
     parts = []
     for dh, dw in taps:
         hs, ws = h + h_pad + dh, w + dw
-        ok = (hs >= 0) & (hs < He) & (ws >= 0) & (ws < W)
-        src = torch.where(ok, (b * He + hs) * W + ws, torch.zeros_like(tok))
+        ok = (hs >= 0) & (hs < s * He) & (ws >= 0) & (ws < s * W)
+        src = torch.where(ok, (b * He + hs.div(s, rounding_mode="floor")) * W + ws.div(s, rounding_mode="floor"),
+                          torch.zeros_like(tok))
         parts.append(a[src, :cin].double() * ok[:, None])
     return torch.cat(parts, dim=1)
 
 
 def gemm_reference(a, w, *, taps, geom, h_pad=0, bias=None, rowvec=None, rv_div=1, rv_mod=1, res1=None, s_res1=1.0,
-                   res2=None, s_res2=1.0, s_acc=1.0, act=0, tile_n=None, stats=None, rows=None):
-    """fp64 epilogue(tap-GEMM) and its magnitude (|A|.|W| propagated through the epilogue).  ``rows``: token subset."""
+                   res2=None, s_res2=1.0, s_acc=1.0, act=0, tile_n=None, stats=None, rows=None, upsample=False):
+    """fp64 epilogue(tap-GEMM) and its magnitude (|A|.|W| propagated through the epilogue).  ``rows``: token subset;
+    ``upsample``: the taps read the nearest-2x upsampled view of ``a`` (im2col64)."""
     cin = w.shape[1] // len(taps)
-    cols = im2col64(a, cin, taps, geom, h_pad, rows)
+    cols = im2col64(a, cin, taps, geom, h_pad, rows, upsample)
     w64 = w.double()
     acc = cols @ w64.t()
     mag = cols.abs() @ w64.abs().t()
@@ -407,11 +412,13 @@ def sharded_kv(k, v, nb, T, S, C, shards, device):
 # ==================================================================================================================
 # Norms, softmax, im2col
 # ==================================================================================================================
-def layernorm_reference(x, gamma, beta, eps, addvec=None, av_div=1, av_mod=1):
+def layernorm_reference(x, gamma, beta, eps, addvec=None, av_div=1, av_mod=1, rows=None):
+    """fp64 LayerNorm of x [tokens, >= C] (of the token subset ``rows``) and its magnitude."""
     C = gamma.numel()
-    v = x[:, :C].double()
+    tok = torch.arange(x.shape[0], device=x.device) if rows is None else rows
+    v = x[tok, :C].double()
     if addvec is not None:
-        v = v + addvec.double()[(torch.arange(v.shape[0], device=x.device) // av_div) % av_mod][:, :C]
+        v = v + addvec.double()[(tok // av_div) % av_mod][:, :C]
     mean = v.mean(1, keepdim=True)
     rstd = torch.rsqrt(v.var(1, unbiased=False, keepdim=True) + eps)
     g, b = gamma.double(), beta.double()
@@ -420,9 +427,18 @@ def layernorm_reference(x, gamma, beta, eps, addvec=None, av_div=1, av_mod=1):
     return ref, mag
 
 
-def groupnorm_reference(x, frames, tpf, gamma, beta, eps, silu, fps, groups=32, stat_x=None):
-    """fp64 GroupNorm of x [frames * tpf, C] with statistics over fps consecutive frames (over `stat_x` if given)."""
+def groupnorm_reference(x, frames, tpf, gamma, beta, eps, silu, fps, groups=32, stat_x=None, rows=None, moments=None):
+    """fp64 GroupNorm of x [frames * tpf, C] with statistics over fps consecutive frames (over `stat_x` if given).
+    ``rows`` with ``moments`` = fp64 (mean, rstd) [frames / fps, groups]: the token subset ``rows`` only, normalised
+    with those statistics (computed elsewhere over the whole frame set)."""
     C = gamma.numel()
+    if rows is not None:
+        mean, rstd = (m[rows // (fps * tpf)].repeat_interleave(C // groups, dim=1) for m in moments)
+        xs = x[rows, :C].double()
+        g, b = gamma.double(), beta.double()
+        pre = (xs - mean) * rstd * g + b
+        mag = (xs.abs() + mean.abs()) * rstd * g.abs() + b.abs()
+        return (F.silu(pre), 1.2 * mag) if silu else (pre, mag)
     xs = x[:, :C].double().reshape(frames // fps, fps * tpf, groups, C // groups)
     sx = xs if stat_x is None else stat_x[:, :C].double().reshape(xs.shape)
     mean = sx.mean(dim=(1, 3), keepdim=True)

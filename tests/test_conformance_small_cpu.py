@@ -823,37 +823,40 @@ D80_LARGE_QK = 12.0 ** 0.5
 # ==================================================================================================================
 _G = "test_conformance_gpu.py::"
 _S = "test_conformance_small_gpu.py::"
+_P = "test_production_conformance_gpu.py::"
+_STEP, _DEC, _COND, _SESS = (_P + "test_sampler_step_production", _P + "test_decode_production",
+                             _P + "test_condition_and_encode_production", _P + "test_session_production")
 KERNEL_TESTS = {
-    "tapgemm_kernel": [_G + "test_gemm_sweep", _G + "test_gemm_production_conv_sampled"],
-    "attn_spatial_kernel": [_G + "test_attention_spatial_edges", _G + "test_attention_spatial_level0_sampled"],
-    "attn_temporal_kernel": [_G + "test_attention_temporal_conformance", _G + "test_attention_temporal_sharded"],
-    "gn_stats_kernel": [_G + "test_groupnorm_conformance", _G + "test_groupnorm_sums_finalize_sharded"],
-    "gn_apply_kernel": [_G + "test_groupnorm_conformance", _G + "test_groupnorm_sums_finalize_sharded"],
+    "tapgemm_kernel": [_G + "test_gemm_sweep", _G + "test_gemm_production_conv_sampled", _STEP, _DEC, _COND],
+    "attn_spatial_kernel": [_G + "test_attention_spatial_edges", _G + "test_attention_spatial_level0_sampled", _STEP],
+    "attn_temporal_kernel": [_G + "test_attention_temporal_conformance", _G + "test_attention_temporal_sharded", _STEP],
+    "gn_stats_kernel": [_G + "test_groupnorm_conformance", _G + "test_groupnorm_sums_finalize_sharded", _STEP, _COND],
+    "gn_apply_kernel": [_G + "test_groupnorm_conformance", _G + "test_groupnorm_sums_finalize_sharded", _STEP, _DEC],
     "gn_finalize_kernel": [_G + "test_groupnorm_sums_finalize_sharded"],
-    "gn_from_partials_kernel": [_G + "test_groupnorm_from_partials_raw_sums_sharded"],
-    "layernorm_kernel": [_G + "test_layernorm_conformance"],
-    "layernorm40_kernel": [_G + "test_layernorm_conformance"],
-    "softmax_rows_kernel": [_G + "test_softmax_rows_conformance"],
-    "im2col_s2_asym_kernel": [_G + "test_im2col_s2_asym_exact"],
-    "clip_preprocess_kernel": ["test_clip_gpu.py::test_preprocess_matches_oracle"],
-    "sinusoid_embed_kernel": ["test_conditioner_gpu.py::test_sinusoid_embed_matches_formula"],
-    "sampler_prepare_kernel": [_S + "test_sampler_step", _S + "test_sampler_trajectory_and_graph_replay"],
-    "sampler_update_kernel": [_S + "test_sampler_step", _S + "test_sampler_trajectory_and_graph_replay"],
+    "gn_from_partials_kernel": [_G + "test_groupnorm_from_partials_raw_sums_sharded", _STEP, _DEC],
+    "layernorm_kernel": [_G + "test_layernorm_conformance", _STEP, _COND],
+    "layernorm40_kernel": [_G + "test_layernorm_conformance", _STEP],
+    "softmax_rows_kernel": [_G + "test_softmax_rows_conformance", _DEC, _COND],
+    "im2col_s2_asym_kernel": [_G + "test_im2col_s2_asym_exact", _COND],
+    "clip_preprocess_kernel": ["test_clip_gpu.py::test_preprocess_matches_oracle", _COND],
+    "sinusoid_embed_kernel": ["test_conditioner_gpu.py::test_sinusoid_embed_matches_formula", _COND],
+    "sampler_prepare_kernel": [_S + "test_sampler_step", _S + "test_sampler_trajectory_and_graph_replay", _STEP],
+    "sampler_update_kernel": [_S + "test_sampler_step", _S + "test_sampler_trajectory_and_graph_replay", _STEP],
     "conv3x3_small_cin_kernel": [_S + "test_conv3x3_small_cin_edges", _S + "test_conv3x3_small_cin_production",
-                                 _S + "test_conv3x3_small_cin_ignores_nonfinite_pad_channels"],
+                                 _S + "test_conv3x3_small_cin_ignores_nonfinite_pad_channels", _DEC, _COND],
     "time_mix_small_kernel": [_S + "test_time_mix_cases", _S + "test_time_mix_decode_and_session_chunks"],
     "time_mix_small_u8_kernel": [_S + "test_time_mix_cases", _S + "test_time_mix_boundaries",
-                                 _S + "test_time_mix_decode_and_session_chunks"],
-    "rollout_advance_kernel": [_S + "test_rollout_advance"],
+                                 _S + "test_time_mix_decode_and_session_chunks", _DEC],
+    "rollout_advance_kernel": [_S + "test_rollout_advance", _SESS],
     "ensemble_reward_kernel": [_S + "test_ensemble_reward", _S + "test_ensemble_reward_identical_members",
-                               _S + "test_ensemble_reward_back_to_back"],
-    "timestep_embedding_kernel": [_S + "test_timestep_embedding"],
-    "blend_emb_kernel": [_S + "test_blend_emb"],
-    "nchw_to_tokens_kernel": [_S + "test_layout_converters"],
-    "tokens_to_nchw_kernel": [_S + "test_layout_converters"],
-    "im2col_s2_kernel": [_S + "test_im2col_s2"],
-    "upsample2x_kernel": [_S + "test_upsample2x"],
-    "attn_d80_kernel": [_S + "test_attention_d80", _S + "test_attention_d80_identical_keys_and_large_logits"],
+                               _S + "test_ensemble_reward_back_to_back", _SESS],
+    "timestep_embedding_kernel": [_S + "test_timestep_embedding", _STEP],
+    "blend_emb_kernel": [_S + "test_blend_emb", _STEP],
+    "nchw_to_tokens_kernel": [_S + "test_layout_converters", _DEC, _COND],
+    "tokens_to_nchw_kernel": [_S + "test_layout_converters", _COND],
+    "im2col_s2_kernel": [_S + "test_im2col_s2", _STEP],
+    "upsample2x_kernel": [_S + "test_upsample2x", _STEP],
+    "attn_d80_kernel": [_S + "test_attention_d80", _S + "test_attention_d80_identical_keys_and_large_logits", _COND],
 }
 NOT_HELD = {
     "peer_put_kernel": "needs two or more GPUs; test_sharded_gpu.py covers the peer-memory transport",
