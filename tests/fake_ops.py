@@ -36,10 +36,7 @@ def gemm(a, w, out, *, taps=((0, 0),), geom=None, bias=None, rowvec=None, rv_div
             acc = acc + s_res2 * _f(res2)
         out.copy_(acc.to(out.dtype))
         if stats is not None:
-            pad = (-tokens) % 128
-            v = F.pad(acc, (0, 0, 0, pad)).reshape(-1, 32, acc.shape[1])
-            stats[: v.shape[0], :acc.shape[1], 0] = v.sum(dim=1)
-            stats[: v.shape[0], :acc.shape[1], 1] = (v * v).sum(dim=1)
+            _stats_partials(out, stats)
         return out
     tokens = a.shape[0]
     N, K = w.shape
@@ -83,12 +80,23 @@ def gemm(a, w, out, *, taps=((0, 0),), geom=None, bias=None, rowvec=None, rv_div
         acc = acc + s_res2 * _f(res2)
     n_out = out.shape[1]
     out.copy_(acc[:, :n_out].to(out.dtype))
-    if stats is not None:              # column partials per (128-token tile, 32-row quarter) of the fp32 values, like the kernel
-        pad = (-tokens) % 128
-        v = F.pad(acc[:, :n_out], (0, 0, 0, pad)).reshape(-1, 32, n_out)
-        stats[: v.shape[0], :n_out, 0] = v.sum(dim=1)
-        stats[: v.shape[0], :n_out, 1] = (v * v).sum(dim=1)
+    if stats is not None:
+        _stats_partials(out, stats)
     return out
+
+
+def _stats_partials(out, stats):
+    """Column partials per (128-token tile, 32-row quarter) of the stored values, like the kernel: the fp32 sum s over
+    the quarter's n valid rows and the fp32 sum of (x - fl(s / n))^2."""
+    tokens, n_out = out.shape
+    pad = (-tokens) % 128
+    v = F.pad(out.float(), (0, 0, 0, pad)).reshape(-1, 32, n_out)
+    n = (tokens - 32 * torch.arange(v.shape[0])).clamp(0, 32).float()[:, None]
+    s = v.sum(dim=1)
+    m = s / n.clamp_min(1)
+    valid = (torch.arange(32)[None, :] < n)[..., None]
+    stats[: v.shape[0], :n_out, 0] = s
+    stats[: v.shape[0], :n_out, 1] = torch.where(valid, (v - m[:, None]) ** 2, torch.zeros_like(v)).sum(dim=1)
 
 
 class GNWorkspace:
@@ -106,8 +114,10 @@ def groupnorm_scratch(frames, tokens_per_frame, groups=32):
 def groupnorm(x, y, frames, tokens_per_frame, gamma, beta, eps, silu, stats=None, frames_per_stat=1, groups=32, ws=None):
     C = gamma.numel()
     xs = _f(x[:, :C]).reshape(frames // frames_per_stat, frames_per_stat * tokens_per_frame, groups, C // groups)
-    mean = xs.mean(dim=(1, 3), keepdim=True)
-    var = xs.var(dim=(1, 3), unbiased=False, keepdim=True)
+    # statistics in fp64 like the kernel's (fp32 sums of deviations combined in fp64), rounded to fp32
+    x64 = xs.double()
+    mean = x64.mean(dim=(1, 3), keepdim=True).float()
+    var = x64.var(dim=(1, 3), unbiased=False, keepdim=True).float()
     if stats is not None:                        # the kernel's (mean, rstd) output
         stats[..., 0] = mean.reshape(stats.shape[:2])
         stats[..., 1] = torch.rsqrt(var + eps).reshape(stats.shape[:2])
@@ -121,7 +131,7 @@ def groupnorm(x, y, frames, tokens_per_frame, gamma, beta, eps, silu, stats=None
 def groupnorm_from_partials(partials, frames, tokens_per_frame, Cc, eps, stats, frames_per_stat=1, groups=32, raw_sums=None):
     n_stat = frames // frames_per_stat
     rows = frames_per_stat * (tokens_per_frame // 128) * 4
-    p = partials[: n_stat * rows, :Cc].double().reshape(n_stat, rows, groups, Cc // groups, 2).sum(dim=(1, 3))
+    p = partials_raw_sums(partials[: n_stat * rows, :Cc]).reshape(n_stat, rows, groups, Cc // groups, 2).sum(dim=(1, 3))
     if raw_sums is not None:
         raw_sums.copy_(p.reshape(raw_sums.shape))
         return stats
@@ -131,6 +141,13 @@ def groupnorm_from_partials(partials, frames, tokens_per_frame, Cc, eps, stats, 
     stats[..., 0] = mean.float()
     stats[..., 1] = torch.rsqrt(var + eps).float()
     return stats
+
+
+def partials_raw_sums(p):
+    """fp64 (sum x, sum x^2) of full 32-row quarters from their GEMM partials (s, sum of (x - s / 32)^2), as
+    gn_from_partials_kernel forms them: (s, m2 + s^2 / 32)."""
+    p = p.double()
+    return torch.stack([p[..., 0], p[..., 1] + p[..., 0] * p[..., 0] / 32], dim=-1)
 
 
 def groupnorm_apply(x, y, frames, tokens_per_frame, gamma, beta, silu, stats, frames_per_stat=1, groups=32):

@@ -208,7 +208,7 @@ def test_groupnorm_sums_finalize_sharded(ops, world, silu):
     x = (rnd((nb * T * hw, C), 81, dev(), dtype=torch.float32) * 2 + 0.7).half()
     gamma = rnd((C,), 82, dev(), dtype=torch.float32) * 0.1 + 1
     beta = rnd((C,), 83, dev(), dtype=torch.float32) * 0.1
-    ref, mag = groupnorm_reference(x, nb * T, hw, gamma, beta, 1e-5, silu, T)
+    ref, mag, extra = groupnorm_reference(x, nb * T, hw, gamma, beta, 1e-5, silu, T)
     x4 = x.reshape(nb, T, hw, C)
     shards = _shards(T, world)
     total = torch.zeros(nb * G, 2, dtype=torch.float64, device=dev())
@@ -227,11 +227,11 @@ def test_groupnorm_sums_finalize_sharded(ops, world, silu):
         ops.groupnorm_finalize_apply(xr, y, nb * (e - s0), hw, gamma, beta, 1e-5, silu, total, count, st, e - s0, groups=G)
         torch.cuda.synchronize()
         rows = lambda t: t.reshape(nb, T, hw, C)[:, s0:e].reshape(-1, C)
-        assert_conform(y, rows(ref), rows(mag), eps_n, "norm", f"sharded GN W={world} [{s0},{e})")
+        assert_conform(y, rows(ref), rows(mag), eps_n, "norm", f"sharded GN W={world} [{s0},{e})", extra=rows(extra))
         tw = torch.empty(xr.shape, dtype=torch.float16)
         fake_ops.groupnorm_finalize_apply(cpu(xr), tw, nb * (e - s0), hw, cpu(gamma), cpu(beta), 1e-5, silu, cpu(total),
                                           count, None, e - s0, groups=G)
-        assert_conform(tw, cpu(rows(ref)), cpu(rows(mag)), eps_n, "norm", "sharded GN twin")
+        assert_conform(tw, cpu(rows(ref)), cpu(rows(mag)), eps_n, "norm", "sharded GN twin", extra=cpu(rows(extra)))
 
 
 @pytest.mark.parametrize("world", [2, 3])
@@ -239,7 +239,7 @@ def test_groupnorm_from_partials_raw_sums_sharded(ops, world):
     """The same with the statistics taken in the epilogue of the producing GEMM: per rank a STATS GEMM writes its
     output and column partials, groupnorm_from_partials(raw_sums=...) turns them into fp64 sums, the ranks' sums are
     added in rank order and finalised.  Must equal fp64 group_norm over the whole clip of the stored GEMM outputs (the
-    partials hold the values before the fp16 store: rounding noise / sqrt(n), far below the bound)."""
+    partials describe the stored values)."""
     nb, T, hw, Cin, C, G = 2, 9, 128, 64, 320, 32
     x = rnd((nb * T * hw, Cin), 91, dev())
     w = rnd((C, Cin), 92, dev(), scale=Cin ** -0.5)
@@ -261,7 +261,7 @@ def test_groupnorm_from_partials_raw_sums_sharded(ops, world):
         total += sums
         outs.append(o)
     o_full = torch.cat([o.reshape(nb, -1, hw, C) for o in outs], dim=1).reshape(-1, C)
-    ref, mag = groupnorm_reference(o_full, nb * T, hw, gamma, beta, 1e-5, True, T)
+    ref, mag, extra = groupnorm_reference(o_full, nb * T, hw, gamma, beta, 1e-5, True, T)
     count = float(C // G) * hw * T
     eps_n = FAMILY["norm"].c_acc * math.sqrt(T * hw * C // G) * U24
     for (s0, e), o in zip(shards, outs):
@@ -270,7 +270,7 @@ def test_groupnorm_from_partials_raw_sums_sharded(ops, world):
         ops.groupnorm_finalize_apply(o, y, nb * (e - s0), hw, gamma, beta, 1e-5, True, total, count, st, e - s0, groups=G)
         torch.cuda.synchronize()
         rows = lambda t: t.reshape(nb, T, hw, C)[:, s0:e].reshape(-1, C)
-        assert_conform(y, rows(ref), rows(mag), eps_n, "norm", f"from_partials W={world} [{s0},{e})")
+        assert_conform(y, rows(ref), rows(mag), eps_n, "norm", f"from_partials W={world} [{s0},{e})", extra=rows(extra))
 
 
 @pytest.mark.parametrize("world", [2, 3, 4])
@@ -450,12 +450,12 @@ def test_groupnorm_conformance(ops, frames, tpf, C, fps, silu):
         y = ybuf[:, :C]
         ops.groupnorm(xv, y, frames, tpf, gamma, beta, 1e-5, silu, frames_per_stat=fps, ws=ws)
         torch.cuda.synchronize()
-        ref, mag = groupnorm_reference(xv, frames, tpf, gamma, beta, 1e-5, silu, fps)
-        assert_conform(y, ref, mag, eps, "norm", f"groupnorm {frames}x{tpf}x{C} fps {fps} mean {offset}")
+        ref, mag, extra = groupnorm_reference(xv, frames, tpf, gamma, beta, 1e-5, silu, fps)
+        assert_conform(y, ref, mag, eps, "norm", f"groupnorm {frames}x{tpf}x{C} fps {fps} mean {offset}", extra=extra)
         assert bool((ybuf[:, C:] == 5.0).all())
         tw = torch.empty(frames * tpf, C, dtype=torch.float16)
         fake_ops.groupnorm(cpu(xv), tw, frames, tpf, cpu(gamma), cpu(beta), 1e-5, silu, frames_per_stat=fps)
-        assert_conform(tw, cpu(ref), cpu(mag), eps, "norm", "groupnorm twin")
+        assert_conform(tw, cpu(ref), cpu(mag), eps, "norm", "groupnorm twin", extra=cpu(extra))
 
 
 @pytest.mark.parametrize("rows,cols", SOFTMAX_CASES)

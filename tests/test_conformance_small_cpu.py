@@ -826,16 +826,23 @@ _S = "test_conformance_small_gpu.py::"
 _P = "test_production_conformance_gpu.py::"
 _STEP, _DEC, _COND, _SESS = (_P + "test_sampler_step_production", _P + "test_decode_production",
                              _P + "test_condition_and_encode_production", _P + "test_session_production")
+_N = "test_norm_statistics_gpu.py::"
 KERNEL_TESTS = {
-    "tapgemm_kernel": [_G + "test_gemm_sweep", _G + "test_gemm_production_conv_sampled", _STEP, _DEC, _COND],
+    "tapgemm_kernel": [_G + "test_gemm_sweep", _G + "test_gemm_production_conv_sampled", _STEP, _DEC, _COND,
+                       _N + "test_gemm_stats_offset_and_flat", _N + "test_gemm_stats_partial_last_tile"],
     "attn_spatial_kernel": [_G + "test_attention_spatial_edges", _G + "test_attention_spatial_level0_sampled", _STEP],
     "attn_temporal_kernel": [_G + "test_attention_temporal_conformance", _G + "test_attention_temporal_sharded", _STEP],
-    "gn_stats_kernel": [_G + "test_groupnorm_conformance", _G + "test_groupnorm_sums_finalize_sharded", _STEP, _COND],
-    "gn_apply_kernel": [_G + "test_groupnorm_conformance", _G + "test_groupnorm_sums_finalize_sharded", _STEP, _DEC],
-    "gn_finalize_kernel": [_G + "test_groupnorm_sums_finalize_sharded"],
-    "gn_from_partials_kernel": [_G + "test_groupnorm_from_partials_raw_sums_sharded", _STEP, _DEC],
-    "layernorm_kernel": [_G + "test_layernorm_conformance", _STEP, _COND],
-    "layernorm40_kernel": [_G + "test_layernorm_conformance", _STEP],
+    "gn_stats_kernel": [_G + "test_groupnorm_conformance", _G + "test_groupnorm_sums_finalize_sharded", _STEP, _COND,
+                        _N + "test_groupnorm_offset_and_flat", _N + "test_groupnorm_offset_and_flat_decoder_scale",
+                        _N + "test_sharded_offset_and_flat"],
+    "gn_apply_kernel": [_G + "test_groupnorm_conformance", _G + "test_groupnorm_sums_finalize_sharded", _STEP, _DEC,
+                        _N + "test_groupnorm_offset_and_flat", _N + "test_gemm_stats_offset_and_flat",
+                        _N + "test_sharded_offset_and_flat"],
+    "gn_finalize_kernel": [_G + "test_groupnorm_sums_finalize_sharded", _N + "test_sharded_offset_and_flat"],
+    "gn_from_partials_kernel": [_G + "test_groupnorm_from_partials_raw_sums_sharded", _STEP, _DEC,
+                                _N + "test_gemm_stats_offset_and_flat", _N + "test_sharded_offset_and_flat"],
+    "layernorm_kernel": [_G + "test_layernorm_conformance", _STEP, _COND, _N + "test_layernorm_offset_and_flat"],
+    "layernorm40_kernel": [_G + "test_layernorm_conformance", _STEP, _N + "test_layernorm_offset_and_flat"],
     "softmax_rows_kernel": [_G + "test_softmax_rows_conformance", _DEC, _COND],
     "im2col_s2_asym_kernel": [_G + "test_im2col_s2_asym_exact", _COND],
     "clip_preprocess_kernel": ["test_clip_gpu.py::test_preprocess_matches_oracle", _COND],

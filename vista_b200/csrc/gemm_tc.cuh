@@ -51,9 +51,12 @@ struct TGParams {
   int ld_res2_b;
   float s_res2;
   float s_acc;
-  // GroupNorm statistics of the OUTPUT, fused (STATS variants): per (128-token tile, 32-row quarter) column sums and sums
-  // of squares of the stored values, fp32, at stats[((tile * 4 + quarter) * stats_ld + stats_col0 + n) * 2 + {0,1}];
-  // the host guarantees that a tile is 128 consecutive tokens (b200v_gemm checks the box)
+  // GroupNorm statistics of the OUTPUT, fused (STATS variants): per (128-token tile, 32-row quarter) the column sum
+  // s of the stored (rounded) values and their sum of squared deviations from the quarter's mean, sum (x - m)^2 with
+  // m = fl(s fl(1 / n)) over the n valid rows, fp32, at stats[((tile * 4 + quarter) * stats_ld + stats_col0 + n) * 2
+  // + {0,1}].  Deviations, not plain squares: a column whose mean is large next to its spread keeps its variance
+  // (sum x^2 - s^2 / n cancels in fp32).  The host guarantees that a tile is 128 consecutive tokens (b200v_gemm
+  // checks the box)
   float* stats;
   int stats_ld, stats_col0;
 };
@@ -228,7 +231,10 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     if (!valid_own) token_own = 0;
     // phase-B row i of this lane = 8 i + rsub (of the warp's 32)
-    const uint32_t vrows = __ballot_sync(0xffffffffu, valid_own) >> rsub;   // bit 8 i <-> row i
+    const uint32_t vball = __ballot_sync(0xffffffffu, valid_own);
+    const uint32_t vrows = vball >> rsub;   // bit 8 i <-> row i
+    const int n_valid = __popc(vball);          // valid rows of the warp's 32 (STATS: the quarter's count)
+    const float inv_n = n_valid > 0 ? 1.0f / (float)n_valid : 0.f;   // exact for full quarters (32)
     int tok[4], rvrow[4];
     {
       const int rv_own = has_rv ? (token_own / p.rv_div) % p.rv_mod : 0;
@@ -344,30 +350,45 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               o.z = fmaf(p.s_res2, b.x, o.z); o.w = fmaf(p.s_res2, b.y, o.w);
             }
           }
-          if (STATS && ok) {
-            cs[0] += o.x; cs[1] += o.y; cs[2] += o.z; cs[3] += o.w;
-            cq[0] = fmaf(o.x, o.x, cq[0]); cq[1] = fmaf(o.y, o.y, cq[1]);
-            cq[2] = fmaf(o.z, o.z, cq[2]); cq[3] = fmaf(o.w, o.w, cq[3]);
-          }
           char* optr = obase + (long long)tok[i] * p.ldo_b;
           if (f32o) {
             if (ok) *reinterpret_cast<float4*>(optr) = o;
           } else {
             const uint2 pk = make_uint2(pack2(o.x, o.y, bf16), pack2(o.z, o.w, bf16));
             if (ok) *reinterpret_cast<uint2*>(optr) = pk;
+            if (STATS) {                 // the statistics describe the stored values
+              const float2 a = unpack2(pk.x, bf16), b = unpack2(pk.y, bf16);
+              o = make_float4(a.x, a.y, b.x, b.y);
+            }
+          }
+          if (STATS) {
+            v[i] = o;                    // kept for the deviations below
+            if (ok) { cs[0] += o.x; cs[1] += o.y; cs[2] += o.z; cs[3] += o.w; }
           }
         }
         if (STATS) {
-          // rows of one column live in lanes ch, ch + 4, ...: fixed-order butterfly, then lane rsub == 0 holds the sums
-          // over the warp's 32 rows (quarter 2 wg + rh of the tile) and writes them: bit-reproducible
+          // rows of one column live in lanes ch, ch + 4, ...: fixed-order butterflies (the column sums, then the squared
+          // deviations from the quarter's mean), after which lane rsub == 0 holds both over the warp's 32 rows (quarter
+          // 2 wg + rh of the tile) and writes them: bit-reproducible
 #pragma unroll
-          for (int off = 4; off < 32; off <<= 1) {
+          for (int off = 4; off < 32; off <<= 1)
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              cs[q] += __shfl_xor_sync(0xffffffffu, cs[q], off);
-              cq[q] += __shfl_xor_sync(0xffffffffu, cq[q], off);
+            for (int q = 0; q < 4; ++q) cs[q] += __shfl_xor_sync(0xffffffffu, cs[q], off);
+          float mq[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) mq[q] = cs[q] * inv_n;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            if (n_ok && ((vrows >> (8 * i)) & 1u)) {
+              const float dx = v[i].x - mq[0], dy = v[i].y - mq[1], dz = v[i].z - mq[2], dw = v[i].w - mq[3];
+              cq[0] = fmaf(dx, dx, cq[0]); cq[1] = fmaf(dy, dy, cq[1]);
+              cq[2] = fmaf(dz, dz, cq[2]); cq[3] = fmaf(dw, dw, cq[3]);
             }
           }
+#pragma unroll
+          for (int off = 4; off < 32; off <<= 1)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) cq[q] += __shfl_xor_sync(0xffffffffu, cq[q], off);
           if (rsub == 0 && n_ok) {
             float* dst = p.stats + (((long long)m_blk * 4 + wg * 2 + rh) * p.stats_ld + p.stats_col0 + n) * 2;
             *reinterpret_cast<float4*>(dst) = make_float4(cs[0], cq[0], cs[1], cq[1]);

@@ -33,8 +33,11 @@ __device__ __forceinline__ float warp_sum(float v) {
 // ------------------------------------------------------------------------------------------
 // GroupNorm statistics, deterministic.  grid = (chunks, frames); a block walks `chunk` tokens of one
 // frame; thread (row, lane) owns the 8-channel vectors lane, lane+L, ... and keeps per-channel fp32
-// partials; rows are combined in a fixed order in shared memory, groups are summed in fp64 and written
-// as one partial per (frame, chunk, group).  The last block to finish a statistic (ticket counter)
+// sums of d = x - K and d^2 around a pivot K, its first value of the channel: a group whose mean is
+// large next to its spread would lose its variance in fp32 sums of x^2 (E x^2 - mean^2 cancels).  The
+// thread turns them into fp64 raw sums (c K + sum d, c K^2 + 2 K sum d + sum d^2) in shared memory;
+// rows are combined in a fixed order there, groups are summed in fp64 and written as one partial per
+// (frame, chunk, group).  The last block to finish a statistic (ticket counter)
 // adds the partials in a fixed order and writes (mean, rstd): bit-identical from run to run, no
 // floating-point atomics, no memset (the counter resets itself).
 // ------------------------------------------------------------------------------------------
@@ -57,7 +60,7 @@ __global__ void __launch_bounds__(kGnThreads)
 gn_stats_kernel(const __half* __restrict__ x, long long ldx, int tokens_per_frame, int C, int groups,
                 int frames_per_stat, int chunk, int L, int J, float eps, double* __restrict__ partials,
                 int* __restrict__ counters, float* __restrict__ mean_rstd, double* __restrict__ raw_out) {
-  extern __shared__ float sh[];  // [rows][2*C]
+  extern __shared__ double sh[];  // [rows][2*C]
   __shared__ int s_last;
   const int frame = blockIdx.y;
   const int t0 = blockIdx.x * chunk;
@@ -65,13 +68,21 @@ gn_stats_kernel(const __half* __restrict__ x, long long ldx, int tokens_per_fram
   const int nvec = C >> 3;
   const int rows = kGnThreads / L;
   const int lane = threadIdx.x % L, row = threadIdx.x / L;
-  float s[JT][8], q[JT][8];
-#pragma unroll
-  for (int j = 0; j < JT; ++j)
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s[j][i] = q[j][i] = 0.f;
   if (row < rows) {
     const __half* base = x + ((long long)frame * tokens_per_frame) * ldx;
+    const int n_tok = t0 + row < t1 ? (t1 - t0 - row + rows - 1) / rows : 0;   // tokens t0 + row, + rows, ... < t1
+    float s[JT][8], q[JT][8], piv[JT][8];
+    uint4 u0[JT];
+#pragma unroll
+    for (int j = 0; j < JT; ++j) {
+      const int v = lane + j * L;
+      u0[j] = make_uint4(0, 0, 0, 0);
+      if (n_tok > 0 && j < J && v < nvec)
+        u0[j] = __ldg(reinterpret_cast<const uint4*>(base + (long long)(t0 + row) * ldx + v * 8));
+      h8_to_f(u0[j], piv[j]);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) s[j][i] = q[j][i] = 0.f;
+    }
     // 4 tokens per iteration: 4 independent 16-byte loads in flight per thread and vector
     for (int t = t0 + row; t < t1; t += 4 * rows) {
 #pragma unroll
@@ -82,7 +93,7 @@ gn_stats_kernel(const __half* __restrict__ x, long long ldx, int tokens_per_fram
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
             const int tt = t + k * rows;
-            u[k] = tt < t1 ? __ldg(reinterpret_cast<const uint4*>(base + (long long)tt * ldx + v * 8)) : make_uint4(0, 0, 0, 0);
+            u[k] = tt < t1 ? __ldg(reinterpret_cast<const uint4*>(base + (long long)tt * ldx + v * 8)) : u0[j];
           }
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
@@ -90,22 +101,25 @@ gn_stats_kernel(const __half* __restrict__ x, long long ldx, int tokens_per_fram
             h8_to_f(u[k], f);
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
-              s[j][i] += f[i];
-              q[j][i] += f[i] * f[i];
+              const float d = f[i] - piv[j][i];   // a token past t1 reads the pivot: d = 0
+              s[j][i] += d;
+              q[j][i] = fmaf(d, d, q[j][i]);
             }
           }
         }
       }
     }
-    float* mine = sh + (size_t)row * 2 * C;
+    double* mine = sh + (size_t)row * 2 * C;
+    const double cnt = (double)n_tok;
 #pragma unroll
     for (int j = 0; j < JT; ++j) {
       const int v = lane + j * L;
       if (j < J && v < nvec) {
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          mine[v * 8 + i] = s[j][i];
-          mine[C + v * 8 + i] = q[j][i];
+          const double K = (double)piv[j][i], sd = (double)s[j][i];
+          mine[v * 8 + i] = fma(cnt, K, sd);
+          mine[C + v * 8 + i] = fma(cnt * K, K, fma(2.0 * K, sd, (double)q[j][i]));
         }
       }
     }
@@ -116,10 +130,10 @@ gn_stats_kernel(const __half* __restrict__ x, long long ldx, int tokens_per_fram
   for (int g = threadIdx.x; g < groups; g += kGnThreads) {
     double a = 0.0, b = 0.0;
     for (int r = 0; r < rows; ++r) {
-      const float* p = sh + (size_t)r * 2 * C;
+      const double* p = sh + (size_t)r * 2 * C;
       for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
-        a += (double)p[c];
-        b += (double)p[C + c];
+        a += p[c];
+        b += p[C + c];
       }
     }
     double* dst = partials + (((long long)frame * chunks + blockIdx.x) * groups + g) * 2;
@@ -139,7 +153,7 @@ gn_stats_kernel(const __half* __restrict__ x, long long ldx, int tokens_per_fram
   // Final reduction, fixed order: 8 threads per group each add every 8th partial in index order, thread 0 of the
   // group adds the 8 sub-sums in order (the partial count reaches frames_per_stat * chunks ~ 10^3).
   const double cnt = (double)cpg * tokens_per_frame * frames_per_stat;
-  double* red = reinterpret_cast<double*>(sh);   // [groups][8][2]; the row partials in sh are dead by now
+  double* red = sh;   // [groups][8][2]; the row partials in sh are dead by now
   const int n_part = frames_per_stat * chunks;
   for (int idx = threadIdx.x; idx < groups * 8; idx += kGnThreads) {
     const int g = idx >> 3, sub = idx & 7;
@@ -925,7 +939,7 @@ static int gn_stats_impl(const void* x, int64_t ldx, int32_t frames, int32_t tok
   const int rows = kGnThreads / L;
   const int chunk = gn_pick_chunk(frames, tokens_per_frame);
   dim3 grid((tokens_per_frame + chunk - 1) / chunk, frames);
-  size_t smem = (size_t)rows * 2 * C * sizeof(float);
+  size_t smem = (size_t)rows * 2 * C * sizeof(double);
   if (smem < (size_t)groups * 8 * 2 * sizeof(double)) smem = (size_t)groups * 8 * 2 * sizeof(double);
   static bool attr_set[64] = {false};
   if (vb::first_use_on_device(attr_set)) {
@@ -983,8 +997,10 @@ extern "C" int b200v_groupnorm_finalize(const double* sums, int32_t n_stat_group
 }
 
 // (mean, rstd) from the column partials of the producing tap-GEMM (gemm_tc.cu, STATS variants).  grid = (groups, stats);
-// thread t adds partial rows t, t + 256, ... of its group's columns in fp64, the 256 sub-sums are combined by a fixed
-// tree: bit-identical from run to run.
+// a partial is (s, m2) of 32 rows (sum, squared deviations from s / 32: every quarter of a frame's tiles is full, as
+// tokens_per_frame % 128 == 0 and the tiles of a STATS GEMM are whole); thread t adds the raw sums s and m2 + s^2 / 32 of
+// partial rows t, t + 256, ... of its group's columns in fp64, the 256 sub-sums are combined by a fixed tree:
+// bit-identical from run to run.  fp64 sums of x^2 cancel only at ~2^-53 (mean / std)^2 in the finalisation.
 namespace vb {
 __global__ void __launch_bounds__(256)
 gn_from_partials_kernel(const float* __restrict__ partials, long long ld, int rows_per_stat, int cpg, int groups, float eps,
@@ -998,7 +1014,7 @@ gn_from_partials_kernel(const float* __restrict__ partials, long long ld, int ro
     for (int c = 0; c < cpg; ++c) {
       const float2 v = __ldg(row + c);
       a += (double)v.x;
-      b += (double)v.y;
+      b += fma((double)v.x * (1.0 / 32.0), (double)v.x, (double)v.y);
     }
   }
   red[0][threadIdx.x] = a;

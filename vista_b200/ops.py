@@ -157,9 +157,10 @@ def gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, taps: Sequence[
     """out = epilogue(tap-GEMM(a, w)).  ``a``: [tokens, >=cin] fp16 view; ``w``: [N, ntaps*cin] fp16;
     ``geom`` = (W, H, NB) turns on image taps (zero padded); act 1 = SiLU, act 2 = GEGLU (out has N/2 columns),
     act 3 = erf-GELU.
-    ``stats`` = partials [tokens/128*4, N, 2] fp32 (may be a column slice of a wider matrix): the epilogue also writes the
-    column sums / sums of squares of the output (GroupNorm statistics of the consumer without a pass over the tensor);
-    the token tiles are then the 128-consecutive-token ones of stats_box().
+    ``stats`` = partials [tokens/128*4, N, 2] fp32 (may be a column slice of a wider matrix): the epilogue also writes,
+    per 32-row quarter of each token tile, the column sum of the stored output and its sum of squared deviations from
+    the quarter's mean (GroupNorm statistics of the consumer without a pass over the tensor, exact for groups whose
+    mean is large next to their spread); the token tiles are then the 128-consecutive-token ones of stats_box().
     ``h_pad``: ``a`` holds h_pad extra rows of H before and after the H rows of ``geom`` (halo frames of the frame-sharded
     (3,1,1) convolution): ``a`` is the extended [(NB (H + 2 h_pad) W), C] tensor, the output has NB H W rows.
     ``upsample``: the taps run over the nearest-2x upsampled view of ``a`` (``geom`` is the geometry of ``a``; ``out`` and
