@@ -59,8 +59,10 @@ def _ln(sd: SD, p: str, x: torch.Tensor) -> torch.Tensor:
 # ---------------------------------------------------------------------------------------------
 # VideoResBlock
 # ---------------------------------------------------------------------------------------------
-def res_block_2d(sd: SD, p: str, x: torch.Tensor, emb: torch.Tensor, has_skip: bool) -> torch.Tensor:
-    """openaimodel.py:258-284 with dims=2, no up/down, no scale-shift norm. GroupNorm32 eps 1e-5."""
+def res_block_2d(sd: SD, p: str, x: torch.Tensor, emb: torch.Tensor, has_skip: bool, record: Optional[dict] = None
+                 ) -> torch.Tensor:
+    """openaimodel.py:258-284 with dims=2, no up/down, no scale-shift norm. GroupNorm32 eps 1e-5.  ``record``: receives
+    the residual operand as "res2d" (test aid; the arithmetic is the same with or without it)."""
     h = F.conv2d(F.silu(_gn(sd, f"{p}.in_layers.0", x, 1e-5)),
                  sd[f"{p}.in_layers.2.weight"], sd[f"{p}.in_layers.2.bias"], padding=1)
     emb_out = _lin(sd, f"{p}.emb_layers.1", F.silu(emb))
@@ -69,6 +71,8 @@ def res_block_2d(sd: SD, p: str, x: torch.Tensor, emb: torch.Tensor, has_skip: b
                  sd[f"{p}.out_layers.3.weight"], sd[f"{p}.out_layers.3.bias"], padding=1)
     if has_skip:
         x = F.conv2d(x, sd[f"{p}.skip_connection.weight"], sd[f"{p}.skip_connection.bias"])
+    if record is not None:
+        record["res2d"] = x
     return x + h
 
 
@@ -86,14 +90,22 @@ def res_block_3d(sd: SD, p: str, x: torch.Tensor, emb: Optional[torch.Tensor]) -
     return x + h
 
 
-def video_res_block(sd: SD, rb: ResBlockSpec, x: torch.Tensor, emb: torch.Tensor, T: int) -> torch.Tensor:
-    """video_model.py:59-75; blend util.py:311-318: alpha*spatial + (1-alpha)*temporal."""
-    x = res_block_2d(sd, rb.prefix, x, emb, rb.has_skip)
+def video_res_block(sd: SD, rb: ResBlockSpec, x: torch.Tensor, emb: torch.Tensor, T: int,
+                    record: Optional[dict] = None) -> torch.Tensor:
+    """video_model.py:59-75; blend util.py:311-318: alpha*spatial + (1-alpha)*temporal.
+
+    ``record`` (test aid, tests/block_shadow.py): receives every operand added as a residual ("res2d", the spatial
+    block's; "res3d", the temporal block's) and the blend as "blend" = (alpha, a, b) with out = alpha a + (1 - alpha) b,
+    all in the output's (bt, c, h, w) layout.  The arithmetic is the same with or without it."""
+    x = res_block_2d(sd, rb.prefix, x, emb, rb.has_skip, record)
     bt, c, h, w = x.shape
     x5 = x.reshape(bt // T, T, c, h, w).permute(0, 2, 1, 3, 4)
     xt = res_block_3d(sd, f"{rb.prefix}.time_stack", x5, emb.reshape(bt // T, T, -1))
     alpha = torch.sigmoid(sd[f"{rb.prefix}.time_mixer.mix_factor"])
     out = alpha * x5 + (1.0 - alpha) * xt
+    if record is not None:
+        record["res3d"] = x
+        record["blend"] = (alpha, x, xt.permute(0, 2, 1, 3, 4).reshape(bt, c, h, w))
     return out.permute(0, 2, 1, 3, 4).reshape(bt, c, h, w)
 
 
@@ -153,9 +165,10 @@ def video_transformer_block(sd: SD, p: str, x, time_context, heads, ctx_dim, T: 
 
 
 def spatial_video_transformer(sd: SD, t: SVTSpec, x: torch.Tensor, context: torch.Tensor,
-                              T: int, ctx_dim: int) -> torch.Tensor:
+                              T: int, ctx_dim: int, record: Optional[dict] = None) -> torch.Tensor:
     """video_attention.py:239-296 (use_linear, use_spatial_context, depth 1); GroupNorm eps 1e-6
-    (attention.py:141-142)."""
+    (attention.py:141-142).  ``record`` (test aid): receives the residual operand x_in as "res" and the blend as
+    "blend" = (alpha, x, x_mix) in the inner (B, H W, C) layout, before proj_out.  The arithmetic is unchanged."""
     B, C, H, W = x.shape
     p = t.prefix
     x_in = x
@@ -169,6 +182,8 @@ def spatial_video_transformer(sd: SD, t: SVTSpec, x: torch.Tensor, context: torc
     x = basic_transformer_block(sd, f"{p}.transformer_blocks.0", x, context, t.heads, ctx_dim)
     x_mix = video_transformer_block(sd, f"{p}.time_stack.0", x + emb, time_context, t.heads, ctx_dim, T)
     alpha = torch.sigmoid(sd[f"{p}.time_mixer.mix_factor"])
+    if record is not None:
+        record["res"], record["blend"] = x_in, (alpha, x, x_mix)
     x = alpha * x + (1.0 - alpha) * x_mix                            # util.py:317
     x = _lin(sd, f"{p}.proj_out", x)
     x = x.reshape(B, H, W, C).permute(0, 3, 1, 2)
@@ -314,30 +329,41 @@ def _swish(x):
     return x * torch.sigmoid(x)
 
 
-def dec_video_res_block(sd: SD, p: str, x: torch.Tensor, has_skip: bool, T: int) -> torch.Tensor:
+def dec_video_res_block(sd: SD, p: str, x: torch.Tensor, has_skip: bool, T: int,
+                        record: Optional[dict] = None) -> torch.Tensor:
     """temporal_ae.py:55-72 on top of model.py:116-135 (temb=None).  VAE GroupNorm eps 1e-6 for the
-    spatial norms, 1e-5 inside the temporal openaimodel.ResBlock; blend alpha*temporal + (1-alpha)*spatial."""
+    spatial norms, 1e-5 inside the temporal openaimodel.ResBlock; blend alpha*temporal + (1-alpha)*spatial.
+    ``record`` (test aid): "res2d", "res3d" and "blend" = (alpha, a, b), out = alpha a + (1 - alpha) b, as in
+    video_res_block.  The arithmetic is unchanged."""
     h = F.conv2d(_swish(_gn(sd, f"{p}.norm1", x, 1e-6)), sd[f"{p}.conv1.weight"], sd[f"{p}.conv1.bias"], padding=1)
     h = F.conv2d(_swish(_gn(sd, f"{p}.norm2", h, 1e-6)), sd[f"{p}.conv2.weight"], sd[f"{p}.conv2.bias"], padding=1)
     if has_skip:
         x = F.conv2d(x, sd[f"{p}.nin_shortcut.weight"], sd[f"{p}.nin_shortcut.bias"])
+    if record is not None:
+        record["res2d"] = x
     x = x + h
     bt, c, hh, ww = x.shape
     x5 = x.reshape(bt // T, T, c, hh, ww).permute(0, 2, 1, 3, 4)
     xt = res_block_3d(sd, f"{p}.time_stack", x5, None)
     alpha = torch.sigmoid(sd[f"{p}.mix_factor"])
     out = alpha * xt + (1.0 - alpha) * x5
+    if record is not None:
+        record["res3d"] = x
+        record["blend"] = (alpha, xt.permute(0, 2, 1, 3, 4).reshape(bt, c, hh, ww), x)
     return out.permute(0, 2, 1, 3, 4).reshape(bt, c, hh, ww)
 
 
-def dec_attn_block(sd: SD, p: str, x: torch.Tensor) -> torch.Tensor:
-    """model.py:147-176: GN, 1x1 q/k/v, single-head SDPA with d = C, 1x1 proj_out, residual."""
+def dec_attn_block(sd: SD, p: str, x: torch.Tensor, record: Optional[dict] = None) -> torch.Tensor:
+    """model.py:147-176: GN, 1x1 q/k/v, single-head SDPA with d = C, 1x1 proj_out, residual.  ``record`` (test aid):
+    receives the residual operand as "res"."""
     b, c, h, w = x.shape
     hn = _gn(sd, f"{p}.norm", x, 1e-6)
     q, k, v = (F.conv2d(hn, sd[f"{p}.{n}.weight"], sd[f"{p}.{n}.bias"]) for n in ("q", "k", "v"))
     q, k, v = (t.reshape(b, 1, c, h * w).transpose(2, 3) for t in (q, k, v))
     o = F.scaled_dot_product_attention(q, k, v)
     o = o.transpose(2, 3).reshape(b, c, h, w)
+    if record is not None:
+        record["res"] = x
     return x + F.conv2d(o, sd[f"{p}.proj_out.weight"], sd[f"{p}.proj_out.bias"])
 
 
@@ -387,12 +413,15 @@ def decode_first_stage(sd: SD, cfg: DecoderConfig, z: torch.Tensor, scale_factor
 # ---------------------------------------------------------------------------------------------
 # VAE encoder (SURVEY.md §8f rank 1: the next row; oracle first)
 # ---------------------------------------------------------------------------------------------
-def enc_res_block(sd: SD, p: str, x: torch.Tensor, has_skip: bool) -> torch.Tensor:
-    """model.py:116-135 with temb = None (Encoder sets temb_ch = 0, model.py:467)."""
+def enc_res_block(sd: SD, p: str, x: torch.Tensor, has_skip: bool, record: Optional[dict] = None) -> torch.Tensor:
+    """model.py:116-135 with temb = None (Encoder sets temb_ch = 0, model.py:467).  ``record`` (test aid): receives
+    the residual operand as "res"."""
     h = F.conv2d(_swish(_gn(sd, f"{p}.norm1", x, 1e-6)), sd[f"{p}.conv1.weight"], sd[f"{p}.conv1.bias"], padding=1)
     h = F.conv2d(_swish(_gn(sd, f"{p}.norm2", h, 1e-6)), sd[f"{p}.conv2.weight"], sd[f"{p}.conv2.bias"], padding=1)
     if has_skip:
         x = F.conv2d(x, sd[f"{p}.nin_shortcut.weight"], sd[f"{p}.nin_shortcut.bias"])
+    if record is not None:
+        record["res"] = x
     return x + h
 
 

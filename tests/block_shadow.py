@@ -28,6 +28,16 @@ the interior.  Per partition, rel-L2(out, ref) <= C_KIND[kind] x rho, rho the re
 fp16 (the rounding floor of assert_conform; also for the fp32 outputs: net_out, the moments and the frames).
 Conditioning vectors are fp32: they take the GEMM family's element rule, |out - ref| <= ulp32(ref) + eps x mag.
 
+Gain check (tests/bias.py), per layer with a residual or an alpha blend (the UNet's ResBlocks and transformers, the
+decoder's and encoder's ResBlocks and mid attention), per clip: e = out - RN16(ref) is fitted to the residual operands
+the oracle records (``record=``), as they enter the output, and to d out / d alpha (the difference of the two blend
+branches, with the blend's sign; for a transformer mapped through proj_out), with one intercept per (frame, channel) to
+absorb constants rounded once per frame (emb_out, the cross-attention rows), standard errors clustered by frame (by
+128-token tile for one frame).  A term fails above B + 4 sigma, B = U16 / 8: a gain of one rounding in every residual
+add, or an alpha one fp16 ulp off, passes the partition rule and fails this one.  The decoder's ResBlocks accumulate the
+fit band by band with their reference (the temporal residual and d out / d alpha; the spatial residual of their pieces
+is not kept).
+
 Failures are collected per key, one report() prints the census (per layer prefix: kind, output shape, worst partition
 ratio), and assert_ok() raises with every failure."""
 import contextlib
@@ -38,6 +48,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 import torch.nn.functional as F
 
+import bias
 from oracle import vista_oracle as vo
 from test_conformance_cpu import FAMILY, U24, rel_l2, ulp
 from vista_b200 import unet as unet_mod
@@ -99,6 +110,55 @@ POS_ROUNDINGS = 4          # timestep_embedding store, W0, the hidden store, W2
 
 def _acc(K):
     return FAMILY["gemm"].c_acc * math.sqrt(K) * U24
+
+
+# ==================================================================================================================
+# Gain check of a layer
+# ==================================================================================================================
+GAIN_KINDS = {"unet.resblock", "unet.svt", "dec.resblock", "dec.attn", "enc.resblock", "enc.attn"}
+GAIN_B = bias.base_bound(torch.float16)
+
+
+def layer_labels(n, C, rows, W, row0, dev):
+    """(cluster, n_clusters, group, n_groups) of an (n, C, rows, W) piece starting at image row ``row0``: clusters are
+    frames (128-token tiles of the frame when n = 1), the nuisance groups (frame, channel).  ``W`` and the tile count
+    assume rows of width W; n_clusters is an upper bound (unused labels cost nothing)."""
+    group = (torch.arange(n, device=dev)[:, None, None, None] * C + torch.arange(C, device=dev)[None, :, None, None])
+    if n >= 2:
+        return torch.arange(n, device=dev)[:, None, None, None], n, group, n * C
+    tok = (row0 + torch.arange(rows, device=dev))[:, None] * W + torch.arange(W, device=dev)[None, :]
+    return (tok // 128)[None, None], None, group, C
+
+
+def layer_directions(kind, rec, sd, prefix):
+    """name -> fp64 (n, C, H, W) directions of a layer's output from the oracle's record: its residual operands and
+    d out / d alpha = a - b of the blend out = alpha a + (1 - alpha) b (a transformer's through proj_out's weight)."""
+    d = {k: rec[k] for k in ("res", "res2d", "res3d") if k in rec}
+    if "blend" in rec:
+        _, a, b = rec["blend"]
+        diff = a - b
+        if kind == "unet.svt":
+            B_, C, H, W = rec["res"].shape
+            diff = F.linear(diff, sd[f"{prefix}.proj_out.weight"]).reshape(B_, H, W, C).permute(0, 3, 1, 2)
+        d["d_alpha"] = diff
+    return d
+
+
+class LayerGain:
+    """The gain fit of one layer and clip, accumulated piece by piece."""
+
+    def __init__(self, names, n, C, H, W, dev):
+        self.names, self.n, self.C, self.W = list(names), n, C, W
+        n_cl = n if n >= 2 else -(-H * W // 128)
+        self.fit = bias.GainFit(self.names, {k: GAIN_B for k in self.names}, n_cl, n * C, device=dev)
+
+    def add(self, out, ref, dirs, row0=0):
+        cl, _, group, _ = layer_labels(self.n, self.C, ref.shape[2], self.W, row0, ref.device)
+        e = out - bias.rn(ref, torch.float16)
+        self.fit.add(e, [dirs[k] for k in self.names], cl, group, out=ref)
+
+    def result(self):
+        return self.fit.result()
 
 
 # ==================================================================================================================
@@ -183,9 +243,11 @@ def _gn_apply(x, mean, var, gamma, beta, eps, groups):
     return y.reshape(x.shape) * gamma.reshape(bc) + beta.reshape(bc)
 
 
-def dec_video_res_block_pieces(sd, p, frame, T, has_skip, sink, groups=32, band_bytes=BAND_BYTES):
+def dec_video_res_block_pieces(sd, p, frame, T, has_skip, sink, groups=32, band_bytes=BAND_BYTES, with_dirs=False):
     """vista_oracle.dec_video_res_block in pieces.  frame(f) -> fp64 (1, Cin, H, W) of input frame f; sink(ref, r0)
-    receives the output rows r0 : r0 + ref.shape[2] of every frame, ref (T, C, rows, W).
+    receives the output rows r0 : r0 + ref.shape[2] of every frame, ref (T, C, rows, W); ``with_dirs``: sink(ref, r0,
+    dirs) with the band's gain directions, "res3d" (the temporal residual operand) and "d_alpha" (temporal minus
+    spatial branch: the blend is alpha temporal + (1 - alpha) spatial).
     Spatial half (per frame, its GroupNorms are per frame): the oracle's own enc_res_block, the first lines of
     dec_video_res_block.  Temporal half: res_block_3d (GroupNorm over (C/32, T, H, W), eps 1e-5, SiLU, (3,1,1)
     convolutions zero padded over frames) and the blend alpha * temporal + (1 - alpha) * spatial."""
@@ -217,7 +279,11 @@ def dec_video_res_block_pieces(sd, p, frame, T, has_skip, sink, groups=32, band_
                              groups))
         h2 = F.conv3d(a[None], sd[f"{t}.out_layers.3.weight"], sd[f"{t}.out_layers.3.bias"], padding=(1, 0, 0))[0]
         x5 = band(r0, r1)
-        sink((alpha * (x5 + h2) + (1.0 - alpha) * x5).transpose(0, 1), r0)
+        ref = (alpha * (x5 + h2) + (1.0 - alpha) * x5).transpose(0, 1)
+        if with_dirs:
+            sink(ref, r0, {"res3d": x5.transpose(0, 1), "d_alpha": h2.transpose(0, 1)})
+        else:
+            sink(ref, r0)
 
 
 def upconv_pieces(w, b, frame, T, sink):
@@ -390,6 +456,7 @@ class Parts:
 class Census:
     def __init__(self, kind):
         self.kind, self.shape, self.ratio, self.part, self.calls = kind, None, 0.0, None, 0
+        self.gain, self.gain_term = 0.0, None         # worst |beta| / (B + 4 sigma) over its clips, and that term
 
 
 class Run:
@@ -419,8 +486,9 @@ class BlockShadow:
         (vae_mod.EncoderRuntime, ("forward", "_enc_resblock")),
     )
 
-    def __init__(self, unet=None, decoder=None, encoder=None, decoder_layer_calls=None):
+    def __init__(self, unet=None, decoder=None, encoder=None, decoder_layer_calls=None, gain: bool = True):
         self.sd = {"unet": unet, "dec": decoder, "enc": encoder}
+        self.gain = gain              # the gain check of the layers in GAIN_KINDS
         self.decoder_layer_calls = decoder_layer_calls
         self.census: Dict[str, Census] = {}
         self.failures: Dict[tuple, str] = {}
@@ -468,6 +536,16 @@ class BlockShadow:
         if r > 1.0:
             self._fail(("layer", name), f"{name} ({kind}): partition {part} rel-L2 is {r:.2f} x the bound "
                                         f"{c:.2f} rho")
+
+    def _gain_note(self, name, kind, terms, clip):
+        w = bias.worst(terms)
+        e = self.census.setdefault(name, Census(kind))
+        if w is not None and w.ratio >= e.gain:
+            e.gain, e.gain_term = w.ratio, w
+        bad = bias.failures(terms)
+        if bad:
+            self._fail(("gain", name), f"{name} ({kind}), clip {clip}: systematic gain on " +
+                       "; ".join(repr(t) for t in bad))
 
     def _elements(self, name, out, ref, tol):
         err = (out.double() - ref).abs()
@@ -573,14 +651,25 @@ class BlockShadow:
         parts = Parts()
         sdl = self._sdl(net, node.name if kind not in ("dec.attn", "enc.attn") else "mid.attn_1", dev)
         clips = n // T if net == "unet" else 1
+        label = self.label(net, node.name)
         if kind in ("dec.resblock", "dec.upconv"):
             frame = lambda f: nchw(x[f * h * w:(f + 1) * h * w], 1, h, w, C_in)
             yt = y.reshape(T, ho, wo, -1)
-            if kind == "dec.resblock":
+            if kind == "dec.resblock" and not self.gain:
                 sink = lambda ref, r0: parts.add(yt[:, r0:r0 + ref.shape[2], :, :node.cout].permute(0, 3, 1, 2).double(),
                                                  ref, 0, r0, ho)
                 with torch.no_grad():
                     dec_video_res_block_pieces(sdl, node.name, frame, T, node.spec.has_skip, sink)
+            elif kind == "dec.resblock":
+                lg = LayerGain(("res3d", "d_alpha"), T, node.cout, ho, wo, dev)
+
+                def sink(ref, r0, dirs):
+                    yo = yt[:, r0:r0 + ref.shape[2], :, :node.cout].permute(0, 3, 1, 2).double()
+                    parts.add(yo, ref, 0, r0, ho)
+                    lg.add(yo, ref, dirs, r0)
+                with torch.no_grad():
+                    dec_video_res_block_pieces(sdl, node.name, frame, T, node.spec.has_skip, sink, with_dirs=True)
+                self._gain_note(label, kind, lg.result(), 0)
             else:
                 sink = lambda ref, f: parts.add(yt[f:f + 1, :, :, :node.cout].permute(0, 3, 1, 2).double(), ref, f)
                 with torch.no_grad():
@@ -590,20 +679,21 @@ class BlockShadow:
             for c in range(clips):
                 xr = x[c * T * h * w:(c + 1) * T * h * w]
                 xi = nchw(xr, T, h, w, C_in)
+                rec = {} if self.gain and kind in GAIN_KINDS else None
                 if kind == "unet.resblock":
-                    ref = vo.video_res_block(sdl, node.spec, xi, run.emb[c * T:(c + 1) * T], T)
+                    ref = vo.video_res_block(sdl, node.spec, xi, run.emb[c * T:(c + 1) * T], T, record=rec)
                 elif kind == "unet.svt":
                     ref = vo.spatial_video_transformer(sdl, node.spec, xi, run.ctx[c * T:(c + 1) * T], T,
-                                                       run.rt.cfg.context_dim)
+                                                       run.rt.cfg.context_dim, record=rec)
                 elif kind == "unet.down":
                     ref = F.conv2d(xi, sdl[f"{node.name}.weight"], sdl[f"{node.name}.bias"], stride=2, padding=1)
                 elif kind == "unet.up":
                     ref = F.conv2d(F.interpolate(xi, scale_factor=2, mode="nearest"), sdl[f"{node.name}.weight"],
                                    sdl[f"{node.name}.bias"], padding=1)
                 elif kind in ("dec.attn", "enc.attn"):
-                    ref = vo.dec_attn_block(sdl, "mid.attn_1", xi)
+                    ref = vo.dec_attn_block(sdl, "mid.attn_1", xi, record=rec)
                 elif kind == "enc.resblock":
-                    ref = vo.enc_res_block(sdl, node.name, xi, node.spec.has_skip)
+                    ref = vo.enc_res_block(sdl, node.name, xi, node.spec.has_skip, record=rec)
                 elif kind == "enc.down":
                     ref = F.conv2d(F.pad(xi, (0, 1, 0, 1)), sdl[f"{node.name}.weight"], sdl[f"{node.name}.bias"],
                                    stride=2)
@@ -613,9 +703,15 @@ class BlockShadow:
                     raise AssertionError(kind)
                 yo = nchw(y[c * T * ho * wo:(c + 1) * T * ho * wo], T, ho, wo, node.cout)
                 parts.add(yo, ref, c * T)
-                del ref, xi, yo
+                if rec is not None:
+                    dirs = layer_directions(kind, rec, sdl, node.name)
+                    lg = LayerGain(list(dirs), T, node.cout, ho, wo, dev)
+                    lg.add(yo, ref, dirs)
+                    self._gain_note(label, kind, lg.result(), c)
+                    del dirs, lg
+                del ref, xi, yo, rec
         del sdl
-        self._note(self.label(net, node.name), kind, (no * ho * wo, node.cout), parts)
+        self._note(label, kind, (no * ho * wo, node.cout), parts)
         self.checked[net].add(node.name)
         if extra is not None:
             extra()
@@ -908,12 +1004,23 @@ class BlockShadow:
             out[e.kind] = max(out.get(e.kind, 0.0), e.ratio)
         return out
 
-    def report(self) -> str:
-        lines = [f"{'layer':<44}{'kind':<15}{'shape':<18}{'worst ratio':>12}  partition"]
+    def worst_gain_by_kind(self):
+        """kind -> (worst |beta| / (B + 4 sigma), its layer, its term) over the layers the gain check ran on."""
+        out = {}
         for name, e in self.census.items():
-            lines.append(f"{name:<44}{e.kind:<15}{str(e.shape):<18}{e.ratio:>12.3f}  {e.part}")
+            if e.gain_term is not None and e.gain >= out.get(e.kind, (-1.0,))[0]:
+                out[e.kind] = (e.gain, name, e.gain_term)
+        return out
+
+    def report(self) -> str:
+        lines = [f"{'layer':<44}{'kind':<15}{'shape':<18}{'worst ratio':>12}  partition / worst gain term"]
+        for name, e in self.census.items():
+            lines.append(f"{name:<44}{e.kind:<15}{str(e.shape):<18}{e.ratio:>12.3f}  {e.part}"
+                         + ("" if e.gain_term is None else f" / {e.gain_term!r}"))
         lines.append("worst ratio per kind (rel-L2 / (c_kind rho)): " +
                      ", ".join(f"{k} {v:.3f} (c {C_KIND[k]:.2f})" for k, v in sorted(self.worst_by_kind().items())))
+        lines.append("worst gain per kind (|beta| / (B + 4 sigma)): " +
+                     ", ".join(f"{k} {g:.3f} ({n}: {t!r})" for k, (g, n, t) in sorted(self.worst_gain_by_kind().items())))
         if self.vectors:
             lines.append(f"conditioning vectors: {len(self.vectors)} checked, worst error / element bound "
                          f"{max(self.vectors.values()):.3f}")

@@ -15,6 +15,15 @@ statistics reduced over the whole frame set in fp64 chunk by chunk.
 Sample rows hold every boundary class: the four image borders of the first, a middle and the last frame, the first and
 last token, the whole last m-tile of the box the launcher chose, and ``random_rows`` random rows.
 
+After the element and rel-L2 rule, every checked launch of a GEMM, a normalisation, an attention, softmax_rows or a time
+mix also passes the gain check of tests/bias.py (``Shadow(gain=True)``, the default): the error against the correctly
+rounded reference, e = out - RN(ref), regressed on the terms the reference is the sum of (GEMM with act = 0: s_acc acc,
+bias + rowvec and each scaled residual; norms: the normalised values times gamma, and beta; with an activation, and for
+attention and softmax, the whole reference; time mix: each blend branch and the bias), with standard errors clustered
+by 128-token tile (by row, pixel or (frame, head) where those are the unit).  No term may carry a gain above
+B + 4 sigma, B = U_out / 8 (+ (K / 16) 2^-24 on a GEMM's accumulator term): an error under one ulp per element with a
+fixed sign passes the element rule and fails this one.
+
 Failures are collected (key -> message) so that one run reports every failing configuration; ``assert_ok()`` raises
 with all of them.  An entry point that launches a kernel and has neither a checker nor a SHADOW_EXEMPT reason fails
 the run when it is called, and so does an entry point exempted only because nothing calls it (UNCALLED)."""
@@ -25,6 +34,7 @@ import math
 import torch
 import torch.nn.functional as F
 
+import bias
 from test_conformance_cpu import (ATTN_EPS, FAMILY, U24, assert_conform, attention_reference, check_stats,
                                   gemm_reference, layernorm_reference, groupnorm_reference, rel_l2, softmax_reference,
                                   ulp)
@@ -85,6 +95,8 @@ def _sync(t):
 class Entry:
     def __init__(self, op):
         self.op, self.calls, self.checked, self.ratio, self.rel_floor, self.family = op, 0, 0, 0.0, 0.0, None
+        self.gain, self.gain_term = 0.0, None         # worst |beta| / (B + 4 sigma) of the gain check, and its term
+        self.gain_K = None                            # the GEMM depth of that launch
 
 
 class Check:
@@ -115,6 +127,26 @@ class Check:
         floor = rel_l2(ref.to(r16), ref)
         self._note(family, ratio, rel_l2(o, ref) / floor if floor > 0 else 0.0)
         assert_conform(out, ref, mag, eps, family, f"{self.name}{what}", factor=factor, extra=extra)
+
+    def gain(self, out, ref, terms, cluster, what="", K=None, channel_dim=-1):
+        """The gain check (tests/bias.py) of ``out`` on the reference's ``terms`` (name -> fp64 tensor of out's shape),
+        clustered by ``cluster`` (labels broadcastable to out) and, second, by the output's channels (axis
+        ``channel_dim``); ``K``: a GEMM's depth, whose accumulator term ('acc', or 'ref' with an activation) gets the
+        fp32 accumulation allowance."""
+        if not self.shadow.gain_check or out.numel() == 0:
+            return
+        b0 = bias.base_bound(out.dtype)
+        bounds = {n: b0 + (bias.accumulator_allowance(K) if K is not None and n in ("acc", "ref") else 0.0)
+                  for n in terms}
+        d = channel_dim % out.dim()
+        chan = torch.arange(out.shape[d], device=out.device).reshape((-1,) + (1,) * (out.dim() - 1 - d))
+        res = bias.fit(out, ref, terms, bounds, cluster, cluster2=chan)
+        w, e = bias.worst(res), self.entry
+        if w is not None and w.ratio >= e.gain:
+            e.gain, e.gain_term, e.gain_K = w.ratio, w, K
+        bad = bias.failures(res)
+        if bad:
+            raise AssertionError(f"{self.name}{what}: systematic gain on " + "; ".join(repr(t) for t in bad))
 
     def elements(self, out, ref, tol, family, what=""):
         err = (out.double() - ref).abs()
@@ -205,15 +237,19 @@ def _gemm(chk, A, n):
     dev_rows = rows.to(a.device)
     kw = dict(taps=taps, geom=geom, h_pad=h_pad, bias=A["bias"], rowvec=A["rowvec"], rv_div=A["rv_div"],
               rv_mod=A["rv_mod"], s_acc=A["s_acc"], act=act, tile_n=tile_n, rows=dev_rows, upsample=up)
-    ref, mag = gemm_reference(a, w, **kw)
-    for r, s in ((A["res1"], A["s_res1"]), (A["res2"], A["s_res2"])):   # residuals as the kernel reads them: now
-        if r is not None:
+    terms = {}
+    ref, mag = gemm_reference(a, w, **kw, terms=terms)
+    for name, r, s in (("res1", A["res1"], A["s_res1"]), ("res2", A["res2"], A["s_res2"])):   # as the kernel reads
+        if r is not None:                                                                   # them: now
             v = s * r[dev_rows, :n_out].double()
+            terms[name] = v
             ref, mag = ref + v, mag + v.abs()
     eps = FAMILY["gemm"].c_acc * math.sqrt(K) * U24
+    cl = bias.clusters(rows).to(a.device)[:, None]
 
     def compare():
         chk.conform(out[dev_rows, :n_out], ref, mag, eps, "gemm")
+        chk.gain(out[dev_rows, :n_out], ref, terms, cl, K=K)
         if stats is not None:
             pos = {int(t): i for i, t in enumerate(rows.tolist())}
             for m, tr in zip(tiles, tile_rows):
@@ -323,13 +359,15 @@ def _groupnorm(chk, A, n):
     C = gamma.numel()
     mean, var, eabs, ex2 = moments64(x, frames, tpf, C, fps, groups)
     rows = _gn_rows(chk, frames, tpf, n, fps).to(x.device)
+    terms = {}
     ref, mag, extra = groupnorm_reference(x, frames, tpf, gamma, beta, eps, silu, fps, groups, rows=rows,
-                                          moments=(mean, torch.rsqrt(var + eps)))
+                                          moments=(mean, torch.rsqrt(var + eps)), terms=terms)
     stats = A["stats"]
     eps_n = FAMILY["norm"].c_acc * math.sqrt(fps * tpf * C // groups) * U24
 
     def compare():
         chk.conform(y[rows, :C], ref, mag, eps_n, "norm", extra=extra)
+        chk.gain(y[rows, :C], ref, terms, bias.clusters(rows)[:, None])
         if stats is not None:
             check_mean_rstd(chk, stats.double(), mean, var, eps, gn_stats_accumulation(frames, tpf, C), " stats")
     return compare
@@ -377,13 +415,15 @@ def _gn_apply(chk, A, n):
     eps_gn = chk.shadow.stats_eps.get(stats.data_ptr())
     assert eps_gn is not None, f"{chk.name}: statistics not written by groupnorm_from_partials"
     # the output against GroupNorm of the stored tensor with its own fp64 statistics, not the kernel's
+    terms = {}
     ref, mag, extra = groupnorm_reference(x, frames, tpf, gamma, beta, eps_gn, silu, fps, groups, rows=rows,
-                                          moments=(mean, torch.rsqrt(var + eps_gn)))
+                                          moments=(mean, torch.rsqrt(var + eps_gn)), terms=terms)
 
     def compare():
         # the statistics describe the stored values the producing GEMM(s) summed
         check_mean_rstd(chk, got, mean, var, eps_gn, PARTIALS_ACCUMULATION, " statistics")
         chk.conform(y[rows, :C], ref, mag, eps_n, "norm", extra=extra)
+        chk.gain(y[rows, :C], ref, terms, bias.clusters(rows)[:, None])
     return compare
 
 
@@ -391,8 +431,13 @@ def _layernorm(chk, A, n):
     x, y, gamma, beta, eps = A["x"], A["y"], A["gamma"], A["beta"], A["eps"]
     C = gamma.numel()
     rows = sample_rows(chk, x.shape[0], n).to(x.device)
-    ref, mag = layernorm_reference(x, gamma, beta, eps, A["addvec"], A["av_div"], A["av_mod"], rows=rows)
-    return lambda: chk.conform(y[rows, :C], ref, mag, FAMILY["norm"].c_acc * math.sqrt(C) * U24, "norm")
+    terms = {}
+    ref, mag = layernorm_reference(x, gamma, beta, eps, A["addvec"], A["av_div"], A["av_mod"], rows=rows, terms=terms)
+
+    def compare():
+        chk.conform(y[rows, :C], ref, mag, FAMILY["norm"].c_acc * math.sqrt(C) * U24, "norm")
+        chk.gain(y[rows, :C], ref, terms, bias.clusters(rows)[:, None])
+    return compare
 
 
 def _attn_spatial(chk, A, n):
@@ -408,6 +453,10 @@ def _attn_spatial(chk, A, n):
     def compare():
         for i, (r, hd, o, m) in enumerate(refs):
             chk.conform(out[r, hd * 64:(hd + 1) * 64], o, m, ATTN_EPS, "attn", f" (frame, head) {pairs[i]}")
+        got = torch.cat([out[r, hd * 64:(hd + 1) * 64] for r, hd, _, _ in refs])
+        ref = torch.cat([o for _, _, o, _ in refs])
+        ids = torch.cat([i * seq + qrows.cpu() for i in range(len(refs))])        # (pair, 128-row tile) clusters
+        chk.gain(got, ref, {"ref": ref}, bias.clusters(ids)[:, None])
     return compare
 
 
@@ -419,7 +468,13 @@ def _attn_temporal(chk, A, n):
     g = lambda t: t[idx.reshape(-1), :heads * 64].double().reshape(len(pix), T, heads, 64).permute(0, 2, 1, 3)
     o, m = attention_reference(g(q), g(k), g(v), p_normalised=True)
     back = lambda t: t.permute(0, 2, 1, 3).reshape(-1, heads * 64)
-    return lambda: chk.conform(out[idx.reshape(-1), :heads * 64], back(o), back(m), ATTN_EPS, "attn")
+    cl = bias.clusters(torch.arange(len(pix)).repeat_interleave(T), size=1)[:, None]     # one cluster per pixel
+
+    def compare():
+        got = out[idx.reshape(-1), :heads * 64]
+        chk.conform(got, back(o), back(m), ATTN_EPS, "attn")
+        chk.gain(got, back(o), {"ref": back(o)}, cl)
+    return compare
 
 
 def _attn_d80(chk, A, n):
@@ -433,6 +488,9 @@ def _attn_d80(chk, A, n):
     def compare():
         for i, (r, o, m) in zip(imgs, refs):
             chk.conform(out[r, :heads * 80], o, m, ATTN_EPS, "attn", f" image {i}")
+        got = torch.cat([out[r, :heads * 80] for r, _, _ in refs])
+        ref = torch.cat([o for _, o, _ in refs])
+        chk.gain(got, ref, {"ref": ref}, bias.clusters(torch.arange(ref.shape[0]), size=64)[:, None])
     return compare
 
 
@@ -441,7 +499,11 @@ def _softmax(chk, A, n):
     rows = sample_rows(chk, x.shape[0], min(n, 1024)).to(x.device)
     ref, mag = softmax_reference(x[rows])
     cols = x.shape[1]
-    return lambda: chk.conform(y[rows, :cols], ref, mag, FAMILY["softmax"].c_acc * math.sqrt(cols) * U24, "softmax")
+
+    def compare():
+        chk.conform(y[rows, :cols], ref, mag, FAMILY["softmax"].c_acc * math.sqrt(cols) * U24, "softmax")
+        chk.gain(y[rows, :cols], ref, {"ref": ref}, bias.clusters(rows, size=1)[:, None])     # one cluster per row
+    return compare
 
 
 def _conv_small_cin(chk, A, n):
@@ -499,22 +561,26 @@ def _tokens_to_nchw(chk, A, n):
 
 def _time_mix(u8):
     def checker(chk, A, n):
-        x, w, bias, out, blend, T, HW, Cc = (A[s] for s in ("x", "w", "bias", "out", "blend", "T", "HW", "Cc"))
+        x, w, b, out, blend, T, HW, Cc = (A[s] for s in ("x", "w", "bias", "out", "blend", "T", "HW", "Cc"))
         f0, skip = A["out_frame0"], A["skip_frames"]
         keep = A["keep_f32_from"] if u8 else -1
         pix = sample_rows(chk, HW, max(64, n // T), None, [torch.arange(max(0, HW - 256), HW)]).to(x.device)
         P, F_ = len(pix), out.shape[0]
         xs = x[(torch.arange(T, device=x.device)[:, None] * HW + pix[None]).reshape(-1)]
         prev = out.reshape(F_, Cc, HW)[:, :, pix].clone()
-        ref, mag, extra = tmix_reference(xs, w, bias, T, P, prev, f0, blend, skip)
+        terms = {}
+        ref, mag, extra = tmix_reference(xs, w, b, T, P, prev, f0, blend, skip, terms=terms)
         lo, hi = f0 + skip, f0 + T
         k0 = lo if keep < 0 else max(lo, f0 + keep)
+        cl = bias.clusters(pix.cpu()).reshape(1, 1, -1)
 
         def compare():
             got = out.reshape(F_, Cc, HW)[:, :, pix]
             if k0 < hi:
                 chk.conform(got[k0:hi], ref[k0 - lo:], mag[k0 - lo:], TMIX_EPS, "elementwise", " fp32 frames",
                             extra=extra[k0 - lo:])
+                chk.gain(got[k0:hi], ref[k0 - lo:], {n: t[k0 - lo:] for n, t in terms.items()}, cl, " fp32 frames",
+                         channel_dim=1)
             if u8:
                 b = A["out_u8"].reshape(-1, HW, Cc)[lo:hi, pix].permute(0, 2, 1)
                 tol = ulp(ref, torch.float32) + TMIX_EPS * mag + extra
@@ -717,8 +783,8 @@ class Shadow:
     """``with Shadow() as sh: ...`` checks every new launch configuration of the block; ``sh.census`` maps key ->
     Entry(calls, checked, worst error / bound, worst rel-L2 / floor); ``sh.assert_ok()`` raises with every failure."""
 
-    def __init__(self, first_n: int = 1, random_rows: int = 2048, ops_module=None):
-        self.first_n, self.random_rows = first_n, random_rows
+    def __init__(self, first_n: int = 1, random_rows: int = 2048, ops_module=None, gain: bool = True):
+        self.first_n, self.random_rows, self.gain_check = first_n, random_rows, gain
         self.ops = ops_module or _ops
         self.census, self.failures, self._saved = {}, {}, {}
         self.stats_eps = {}       # (mean, rstd) buffer -> eps of the groupnorm_from_partials call that wrote it
@@ -789,17 +855,29 @@ class Shadow:
         assert not self.failures, f"{len(self.failures)} launch configuration(s) failed:\n" + "\n".join(self.failures.values())
 
     def families(self):
-        """op -> (distinct keys, checked keys, worst error / bound, worst rel-L2 / floor)."""
+        """op -> (distinct keys, checked keys, worst error / bound, worst rel-L2 / floor, worst gain ratio)."""
         out = {}
         for e in self.census.values():
-            k, c, r, f = out.get(e.op, (0, 0, 0.0, 0.0))
-            out[e.op] = (k + 1, c + (e.checked > 0), max(r, e.ratio), max(f, e.rel_floor))
+            k, c, r, f, g = out.get(e.op, (0, 0, 0.0, 0.0, 0.0))
+            out[e.op] = (k + 1, c + (e.checked > 0), max(r, e.ratio), max(f, e.rel_floor), max(g, e.gain))
         return out
 
+    def worst_gain(self, op):
+        """The Term with the worst gain ratio over the keys of ``op`` (None if no gain check ran)."""
+        e = self._worst_gain_entry(op)
+        return None if e is None else e.gain_term
+
+    def _worst_gain_entry(self, op):
+        es = [e for e in self.census.values() if e.op == op and e.gain_term is not None]
+        return max(es, key=lambda e: e.gain_term.ratio) if es else None
+
     def report(self) -> str:
-        lines = [f"{'op':<26}{'keys':>6}{'checked':>9}{'worst err/bound':>17}{'worst rel/floor':>17}"]
-        for op, (k, c, r, f) in sorted(self.families().items()):
-            lines.append(f"{op:<26}{k:>6}{c:>9}{r:>17.3f}{f:>17.3f}")
+        lines = [f"{'op':<26}{'keys':>6}{'checked':>9}{'worst err/bound':>17}{'worst rel/floor':>17}"
+                 f"{'worst |b|/bound':>17}  worst gain term"]
+        for op, (k, c, r, f, g) in sorted(self.families().items()):
+            e = self._worst_gain_entry(op)
+            t = "" if e is None else repr(e.gain_term) + ("" if e.gain_K is None else f" at K = {e.gain_K}")
+            lines.append(f"{op:<26}{k:>6}{c:>9}{r:>17.3f}{f:>17.3f}{g:>17.3f}  {t}")
         lines.append(f"{len(self.census)} keys, {sum(e.calls for e in self.census.values())} calls, "
                      f"{len(self.failures)} failing")
         return "\n".join(lines)

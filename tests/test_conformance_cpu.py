@@ -259,9 +259,13 @@ def im2col64(a, cin, taps, geom, h_pad, rows=None, upsample=False):
 
 
 def gemm_reference(a, w, *, taps, geom, h_pad=0, bias=None, rowvec=None, rv_div=1, rv_mod=1, res1=None, s_res1=1.0,
-                   res2=None, s_res2=1.0, s_acc=1.0, act=0, tile_n=None, stats=None, rows=None, upsample=False):
+                   res2=None, s_res2=1.0, s_acc=1.0, act=0, tile_n=None, stats=None, rows=None, upsample=False,
+                   terms=None):
     """fp64 epilogue(tap-GEMM) and its magnitude (|A|.|W| propagated through the epilogue).  ``rows``: token subset;
-    ``upsample``: the taps read the nearest-2x upsampled view of ``a`` (im2col64)."""
+    ``upsample``: the taps read the nearest-2x upsampled view of ``a`` (im2col64).  ``terms`` (a dict) receives the
+    terms the output is the sum of, for the gain check of tests/bias.py: with act = 0 'acc' (s_acc acc), 'bias'
+    (s_acc bias + rowvec), 'res1' and 'res2' (each times its scale); with an activation the activated part as 'ref'
+    beside the residuals."""
     cin = w.shape[1] // len(taps)
     cols = im2col64(a, cin, taps, geom, h_pad, rows, upsample)
     w64 = w.double()
@@ -277,23 +281,32 @@ def gemm_reference(a, w, *, taps, geom, h_pad=0, bias=None, rowvec=None, rv_div=
         gl = F.gelu(gate)
         ref = (val * gl).reshape(acc.shape[0], N // 2)
         mag = (tm[:, :, 0] * gl.abs() + val.abs() * 1.2 * tm[:, :, 1] + val.abs()).reshape(acc.shape[0], N // 2)
+        if terms is not None:
+            terms["ref"] = ref
         return ref, mag
-    o = s_acc * (acc + b)
+    t = {"acc": s_acc * acc}
+    if bias is not None:
+        t["bias"] = s_acc * b
+    o = t["acc"] + s_acc * b
     mag = abs(s_acc) * (mag + b.abs())
     if rowvec is not None:
         rvv = rowvec.double()[(tok // rv_div) % rv_mod]
+        t["bias"] = t.get("bias", 0) + rvv
         o = o + rvv
         mag = mag + rvv.abs()
     if act == 1:
         o, mag = F.silu(o), 1.2 * mag
     elif act == 3:
         o, mag = F.gelu(o), 1.2 * mag
-    if res1 is not None:
-        r = s_res1 * res1[tok].double()
-        o, mag = o + r, mag + r.abs()
-    if res2 is not None:
-        r = s_res2 * res2[tok].double()
-        o, mag = o + r, mag + r.abs()
+    if act != 0:
+        t = {"ref": o}
+    for name, res, sc in (("res1", res1, s_res1), ("res2", res2, s_res2)):
+        if res is not None:
+            r = sc * res[tok].double()
+            t[name] = r
+            o, mag = o + r, mag + r.abs()
+    if terms is not None:
+        terms.update(t)
     return o, mag
 
 
@@ -426,8 +439,9 @@ def sharded_kv(k, v, nb, T, S, C, shards, device):
 # ==================================================================================================================
 # Norms, softmax, im2col
 # ==================================================================================================================
-def layernorm_reference(x, gamma, beta, eps, addvec=None, av_div=1, av_mod=1, rows=None):
-    """fp64 LayerNorm of x [tokens, >= C] (of the token subset ``rows``) and its magnitude."""
+def layernorm_reference(x, gamma, beta, eps, addvec=None, av_div=1, av_mod=1, rows=None, terms=None):
+    """fp64 LayerNorm of x [tokens, >= C] (of the token subset ``rows``) and its magnitude.  ``terms`` receives the
+    normalised values times gamma as 'norm' and 'beta' (tests/bias.py)."""
     C = gamma.numel()
     tok = torch.arange(x.shape[0], device=x.device) if rows is None else rows
     v = x[tok, :C].double()
@@ -436,12 +450,16 @@ def layernorm_reference(x, gamma, beta, eps, addvec=None, av_div=1, av_mod=1, ro
     mean = v.mean(1, keepdim=True)
     rstd = torch.rsqrt(v.var(1, unbiased=False, keepdim=True) + eps)
     g, b = gamma.double(), beta.double()
-    ref = (v - mean) * rstd * g + b
+    nrm = (v - mean) * rstd * g
+    ref = nrm + b
     mag = (v.abs() + mean.abs()) * rstd * g.abs() + b.abs()
+    if terms is not None:
+        terms.update(norm=nrm, beta=b.expand_as(nrm))
     return ref, mag
 
 
-def groupnorm_reference(x, frames, tpf, gamma, beta, eps, silu, fps, groups=32, stat_x=None, rows=None, moments=None):
+def groupnorm_reference(x, frames, tpf, gamma, beta, eps, silu, fps, groups=32, stat_x=None, rows=None, moments=None,
+                        terms=None):
     """fp64 GroupNorm of x [frames * tpf, C] with statistics over fps consecutive frames (over `stat_x` if given), its
     magnitude and an extra absolute term (assert_conform's ``mag`` and ``extra``).  ``rows`` with ``moments`` = fp64
     (mean, rstd) [frames / fps, groups]: the token subset ``rows`` only, normalised with those statistics (computed
@@ -451,13 +469,16 @@ def groupnorm_reference(x, frames, tpf, gamma, beta, eps, silu, fps, groups=32, 
     statistics and the normalisation in fp32), extra = 4 ulp32(mean) rstd |gamma| (the fp32 mean, and the fp32 terms
     x rstd gamma and beta - mean rstd gamma of an fp32 apply, each of size |mean| rstd |gamma|, rounded: a few ulps of
     the mean, scaled); SiLU's slope is below 1.2.  Nothing grows with |mean| / std: a kernel
-    that loses the variance of an offset or near-flat group to E x^2 - mean^2 in fp32 fails it."""
+    that loses the variance of an offset or near-flat group to E x^2 - mean^2 in fp32 fails it.
+
+    ``terms`` receives what the output is the sum of (tests/bias.py): 'norm' (the normalised values times gamma) and
+    'beta'; with SiLU the whole output as 'ref'."""
     C = gamma.numel()
     g, b = gamma.double(), beta.double()
     if rows is not None:
         mean, rstd = (m[rows // (fps * tpf)].repeat_interleave(C // groups, dim=1) for m in moments)
         xs = x[rows, :C].double()
-        pre = (xs - mean) * rstd * g + b
+        nrm = (xs - mean) * rstd * g
         mag = (xs - mean).abs() * rstd * g.abs() + b.abs()
         extra = 4 * ulp(mean, torch.float32) * rstd * g.abs()
     else:
@@ -465,11 +486,16 @@ def groupnorm_reference(x, frames, tpf, gamma, beta, eps, silu, fps, groups=32, 
         sx = xs if stat_x is None else stat_x[:, :C].double().reshape(xs.shape)
         mean = sx.mean(dim=(1, 3), keepdim=True)
         rstd = torch.rsqrt(sx.var(dim=(1, 3), unbiased=False, keepdim=True) + eps)
-        pre = ((xs - mean) * rstd).reshape(-1, C) * g + b
+        nrm = ((xs - mean) * rstd).reshape(-1, C) * g
         mag = ((xs - mean).abs() * rstd).reshape(-1, C) * g.abs() + b.abs()
         extra = (4 * ulp(mean, torch.float32) * rstd).expand(xs.shape).reshape(-1, C) * g.abs()
+    pre = nrm + b
     if silu:
+        if terms is not None:
+            terms["ref"] = F.silu(pre)
         return F.silu(pre), 1.2 * mag, 1.2 * extra
+    if terms is not None:
+        terms.update(norm=nrm, beta=b.expand_as(nrm))
     return pre, mag, extra
 
 

@@ -348,33 +348,38 @@ def tmix_weights(device, seed, bias=True):
     return w, (randn((3,), seed + 1, device, 0.1) if bias else None)
 
 
-def tmix_reference(x, w, bias, T, HW, prev, out_frame0, blend, skip):
+def tmix_reference(x, w, bias, T, HW, prev, out_frame0, blend, skip, terms=None):
     """fp64 AE3DConv time mix, 3 -> 3 channels, kernel (3,1,1), zero padded over frames, of the token-major fp32 x
     [T HW, >= 3], as NCHW frames [T, 3, HW], then the chunk-overlap blend: frames with blend[t] != 0 are
     0.5 (prev + mix) with `prev` the fp32 frames `out` held before the call.  Returns (ref, mag, extra) for
-    frames skip..T-1: mag = sum |w||x| + |b| (halved when blended), extra = half an ulp of the blend's sum."""
+    frames skip..T-1: mag = sum |w||x| + |b| (halved when blended), extra = half an ulp of the blend's sum.  ``terms``
+    receives the blend's branches (tests/bias.py): 'mix' (the taps), 'bias' and 'prev', each as it enters the output."""
     C = 3
     v = x[:, :C].double().reshape(T, HW, C)
     w64 = w.double()
     acc = torch.zeros(T, HW, C, dtype=torch.float64, device=x.device)
     mag = torch.zeros_like(acc)
-    if bias is not None:
-        acc += bias.double()
-        mag += bias.double().abs()
     for kt in range(3):
         for t in range(T):
             tt = t + kt - 1
             if 0 <= tt < T:
                 acc[t] += v[tt] @ w64[:, :, kt].t()
                 mag[t] += v[tt].abs() @ w64[:, :, kt].abs().t()
-    acc, mag = acc.permute(0, 2, 1)[skip:], mag.permute(0, 2, 1)[skip:]
+    mix = acc.permute(0, 2, 1)[skip:]
+    b = torch.zeros_like(mix) if bias is None else bias.double().reshape(1, C, 1).expand_as(mix)
+    acc, mag = mix + b, (mag.permute(0, 2, 1)[skip:] + b.abs())
     extra = torch.zeros_like(acc)
+    p = torch.zeros_like(acc)
+    half = torch.ones_like(acc[:, :1, :1])
     if blend is not None:
         bl = blend.bool()[skip:].reshape(-1, 1, 1)
-        p = prev.reshape(prev.shape[0], C, HW)[out_frame0 + skip:out_frame0 + T].double()
+        p = torch.where(bl, prev.reshape(prev.shape[0], C, HW)[out_frame0 + skip:out_frame0 + T].double(), p)
         extra = torch.where(bl, 0.5 * ulp(p.abs() + acc.abs(), torch.float32), extra)
+        half = torch.where(bl, 0.5, 1.0)
         acc = torch.where(bl, 0.5 * (p + acc), acc)
         mag = torch.where(bl, 0.5 * mag, mag)
+    if terms is not None:
+        terms.update(mix=half * mix, bias=half * b, prev=0.5 * p)
     return acc, mag, extra
 
 
@@ -827,20 +832,22 @@ _P = "test_production_conformance_gpu.py::"
 _STEP, _DEC, _COND, _SESS = (_P + "test_sampler_step_production", _P + "test_decode_production",
                              _P + "test_condition_and_encode_production", _P + "test_session_production")
 _N = "test_norm_statistics_gpu.py::"
+_B = "test_bias_conformance_gpu.py::"
+_BIAS = [_B + "test_production_keys_clean", _B + "test_planted_defect_fails_the_gain_check"]
 KERNEL_TESTS = {
     "tapgemm_kernel": [_G + "test_gemm_sweep", _G + "test_gemm_production_conv_sampled", _STEP, _DEC, _COND,
-                       _N + "test_gemm_stats_offset_and_flat", _N + "test_gemm_stats_partial_last_tile"],
-    "attn_spatial_kernel": [_G + "test_attention_spatial_edges", _G + "test_attention_spatial_level0_sampled", _STEP],
+                       _N + "test_gemm_stats_offset_and_flat", _N + "test_gemm_stats_partial_last_tile"] + _BIAS,
+    "attn_spatial_kernel": [_G + "test_attention_spatial_edges", _G + "test_attention_spatial_level0_sampled", _STEP] + _BIAS,
     "attn_temporal_kernel": [_G + "test_attention_temporal_conformance", _G + "test_attention_temporal_sharded", _STEP],
     "gn_stats_kernel": [_G + "test_groupnorm_conformance", _G + "test_groupnorm_sums_finalize_sharded", _STEP, _COND,
                         _N + "test_groupnorm_offset_and_flat", _N + "test_groupnorm_offset_and_flat_decoder_scale",
                         _N + "test_sharded_offset_and_flat"],
     "gn_apply_kernel": [_G + "test_groupnorm_conformance", _G + "test_groupnorm_sums_finalize_sharded", _STEP, _DEC,
                         _N + "test_groupnorm_offset_and_flat", _N + "test_gemm_stats_offset_and_flat",
-                        _N + "test_sharded_offset_and_flat"],
+                        _N + "test_sharded_offset_and_flat"] + _BIAS,
     "gn_finalize_kernel": [_G + "test_groupnorm_sums_finalize_sharded", _N + "test_sharded_offset_and_flat"],
     "gn_from_partials_kernel": [_G + "test_groupnorm_from_partials_raw_sums_sharded", _STEP, _DEC,
-                                _N + "test_gemm_stats_offset_and_flat", _N + "test_sharded_offset_and_flat"],
+                                _N + "test_gemm_stats_offset_and_flat", _N + "test_sharded_offset_and_flat"] + _BIAS,
     "layernorm_kernel": [_G + "test_layernorm_conformance", _STEP, _COND, _N + "test_layernorm_offset_and_flat"],
     "layernorm40_kernel": [_G + "test_layernorm_conformance", _STEP, _N + "test_layernorm_offset_and_flat"],
     "softmax_rows_kernel": [_G + "test_softmax_rows_conformance", _DEC, _COND],
@@ -853,7 +860,7 @@ KERNEL_TESTS = {
                                  _S + "test_conv3x3_small_cin_ignores_nonfinite_pad_channels", _DEC, _COND],
     "time_mix_small_kernel": [_S + "test_time_mix_cases", _S + "test_time_mix_decode_and_session_chunks"],
     "time_mix_small_u8_kernel": [_S + "test_time_mix_cases", _S + "test_time_mix_boundaries",
-                                 _S + "test_time_mix_decode_and_session_chunks", _DEC],
+                                 _S + "test_time_mix_decode_and_session_chunks", _DEC] + _BIAS,
     "rollout_advance_kernel": [_S + "test_rollout_advance", _SESS],
     "ensemble_reward_kernel": [_S + "test_ensemble_reward", _S + "test_ensemble_reward_identical_members",
                                _S + "test_ensemble_reward_back_to_back", _SESS],
