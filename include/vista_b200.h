@@ -222,6 +222,9 @@ int b200v_blend_emb(const float* e_plain, const float* e_cond, const float* labe
  *            row t of net_img (the conditional rows with the action slots of crossattn zeroed),
  *            D = D_u + scales[t]*(D_img - D_u) + action_scales[t]*(D_c - D_img); then the Euler step
  *            (coefs == d_prev == NULL) or the 2M step (both given), as in update / update_2m
+ *   update_cond: the unguided step (guidance weight 1): net_c holds the T conditional rows only,
+ *            D = c_skip*x + c_out*net_c; then the Euler step (coefs == d_prev == NULL) or the 2M step
+ *            (both given, D written to d_prev), as in update_action
  * ---------------------------------------------------------------------------------------------- */
 int b200v_sampler_prepare(float* x, const float* cond_frame, const float* mask,
                           const float* concat_u /* uncond rows (T,4,h,w) or NULL = zeros */,
@@ -243,6 +246,11 @@ int b200v_sampler_update_action(float* x, const float* net_out /* as in b200v_sa
                                 const float* coefs /* as in update_2m, or NULL */, float* d_prev /* or NULL */,
                                 const float* sigmas, int32_t* step_idx, int32_t num_steps, int32_t T, int32_t h,
                                 int32_t w, void* stream);
+int b200v_sampler_update_cond(float* x, const float* net_c /* [T*h*w, ld_net] fp32 token-major, 4 channels used */,
+                              int64_t ld_net, const float* cond_frame, const float* mask,
+                              const float* coefs /* as in update_2m, or NULL */, float* d_prev /* or NULL */,
+                              const float* sigmas, int32_t* step_idx, int32_t num_steps, int32_t T, int32_t h,
+                              int32_t w, void* stream);
 
 /* VAE decoder helpers.
  *   softmax_rows : fp32 scores -> fp16 probabilities, one row per block (mid.attn_1 single-head d=512

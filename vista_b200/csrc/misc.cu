@@ -881,6 +881,48 @@ __global__ void sampler_update_kernel(float* __restrict__ x, const float* __rest
     x[idx] = xn;
   }
 }
+// The unguided step (vista_b200.diffusion.IntervalCFG outside its interval, IdentityGuider): net_c holds the T conditional
+// rows only, and D = D_c = c_skip x + c_out net_c, which is what every fused guider gives at guidance weight 1.  Then the
+// Euler step (kMultistep false) or the 2M step as above; the 2M step writes D to d_prev, so a sample that crosses the
+// interval's boundary carries the previous step's D whichever update wrote it.
+template <bool kMultistep>
+__global__ void sampler_update_kernel(float* __restrict__ x, const float* __restrict__ net_c, long long ld_net,
+                                      const float* __restrict__ cond_frame, const float* __restrict__ mask,
+                                      const float* __restrict__ sigmas, const int* __restrict__ step_idx, int num_steps,
+                                      int T, int h, int w, const float4* __restrict__ coefs, float* __restrict__ d_prev) {
+  const int step = *step_idx;
+  const float sigma = sigmas[step], sigma_next = sigmas[step + 1];
+  const float c_skip = 1.0f / (sigma * sigma + 1.0f);
+  const float c_out = -sigma * rsqrtf(sigma * sigma + 1.0f);
+  const int hw = h * w;
+  const long long total = (long long)T * hw;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int t = (int)(i / hw), pix = (int)(i % hw);
+  const float4 nc = *reinterpret_cast<const float4*>(net_c + ((long long)t * hw + pix) * ld_net);
+  const float cn[4] = {nc.x, nc.y, nc.z, nc.w};
+  const bool final_step = (step + 1 == num_steps);
+  const float m = mask ? mask[t] : 0.f;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    const long long idx = ((long long)t * 4 + c) * hw + pix;
+    const float xv = x[idx];
+    const float den = cn[c] * c_out + xv * c_skip;
+    float xn;
+    if constexpr (kMultistep) {
+      const float4 k = coefs[step];
+      float dd = k.z * den;
+      if (k.w != 0.f) dd -= k.w * d_prev[idx];
+      xn = k.x * xv - k.y * dd;
+      d_prev[idx] = den;
+    } else {
+      const float d = (xv - den) / sigma;
+      xn = xv + d * (sigma_next - sigma);
+    }
+    if (final_step && mask && cond_frame) xn = xn * (1.f - m) + cond_frame[idx] * m;
+    x[idx] = xn;
+  }
+}
 __global__ void step_inc_kernel(int* step_idx) { *step_idx += 1; }
 
 // ------------------------------------------------------------------------------------------
@@ -1317,6 +1359,29 @@ extern "C" int b200v_sampler_update_action(float* x, const float* net_out, int64
     sampler_update_kernel<false, true><<<grid, 256, 0, (cudaStream_t)stream>>>(
         x, net_out, cond_frame, mask, scales, sigmas, step_idx, num_steps, T, h, w, ld_net, nullptr, nullptr, net_img,
         ld_img, action_scales);
+  step_inc_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_idx);
+  VB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b200v_sampler_update_cond(float* x, const float* net_c, int64_t ld_net, const float* cond_frame,
+                                         const float* mask, const float* coefs, float* d_prev, const float* sigmas,
+                                         int32_t* step_idx, int32_t num_steps, int32_t T, int32_t h, int32_t w,
+                                         void* stream) {
+  VB_REQUIRE(x && net_c && sigmas && step_idx, "sampler_update_cond: null pointer");
+  VB_REQUIRE(ld_net >= 4 && ld_net % 4 == 0, "sampler_update_cond: ld_net must be a multiple of 4");
+  VB_REQUIRE((coefs == nullptr) == (d_prev == nullptr),
+             "sampler_update_cond: coefs and d_prev are both NULL (Euler) or both given (2M)");
+  VB_REQUIRE(((uintptr_t)coefs & 15) == 0, "sampler_update_cond: coefs must be 16-byte aligned");
+  const long long total = (long long)T * h * w;
+  const unsigned grid = (unsigned)((total + 255) / 256);
+  if (coefs)
+    sampler_update_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(
+        x, net_c, ld_net, cond_frame, mask, sigmas, step_idx, num_steps, T, h, w,
+        reinterpret_cast<const float4*>(coefs), d_prev);
+  else
+    sampler_update_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(
+        x, net_c, ld_net, cond_frame, mask, sigmas, step_idx, num_steps, T, h, w, nullptr, nullptr);
   step_inc_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_idx);
   VB_CHECK_CUDA(cudaGetLastError());
   return 0;

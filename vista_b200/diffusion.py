@@ -8,6 +8,7 @@ Mirrors (paths relative to the reference root):
   Denoiser ................. vwm/modules/diffusionmodules/denoiser.py:10-35
   VanillaCFG / Identity / Linear / TrianglePredictionGuider ... guiders.py
   ActionCFG ................ a separate guidance scale for the action (not in Vista; InstructPix2Pix's two-scale CFG)
+  IntervalCFG .............. guidance on a sigma interval only (not in Vista; Kynkäänniemi et al. 2024)
   EulerEDMSampler .......... vwm/modules/diffusionmodules/sampling.py:15-124
   DPMPP2MSampler ........... sgm's sampling.py DPMPP2MSampler (Vista does not ship it), on the same loop
   instantiate_from_config .. vwm/util.py:154-173
@@ -229,6 +230,8 @@ class ActionCFG(Guider):
     def __init__(self, action_scale: float, guider_config: Dict, context_dim: int = 1024):
         self.action_scale = float(action_scale)
         self.image_guider = instantiate_from_config(guider_config)
+        if isinstance(self.image_guider, IntervalCFG):
+            raise ValueError("IntervalCFG must be the outermost guider: wrap ActionCFG in it, not the other way round")
         self.context_dim = context_dim
         self.additional_cond_keys = list(self.image_guider.additional_cond_keys)
 
@@ -266,6 +269,46 @@ class ActionCFG(Guider):
     def action_scale_vector(self, num_frames):
         """Per-frame s_act (fused path): ``action_scale`` on every frame."""
         return torch.full((num_frames,), self.action_scale)
+
+
+class IntervalCFG(Guider):
+    """Limited-interval guidance (Kynkäänniemi et al. 2024, arXiv 2404.07724): the wrapped guider on the steps whose
+    sigma lies in (sigma_lo, sigma_hi], guidance weight 1 on every other step.  At weight 1 each guider it may wrap
+    (VanillaCFG, Linear- or TrianglePredictionGuider, ActionCFG) gives D = D_c, so an unguided step evaluates the
+    network on the T conditional rows only, half the rows of a CFG step.
+
+    Whether a step is guided is decided per call from its sigma (the value of the fp32 sigma table the sampler reads):
+    ``prepare_inputs`` is the wrapped guider's inside the interval and passes ``(x, s, c, cond_mask)`` through outside
+    it; ``__call__`` is the wrapped guider inside and the identity outside.  It must be the outermost guider."""
+
+    GUIDERS = (VanillaCFG, LinearPredictionGuider, ActionCFG)
+
+    def __init__(self, sigma_lo: float, sigma_hi: float, guider_config: Dict):
+        self.sigma_lo, self.sigma_hi = float(sigma_lo), float(sigma_hi)
+        if not self.sigma_lo < self.sigma_hi:
+            raise ValueError(f"IntervalCFG: sigma_lo ({sigma_lo}) must be below sigma_hi ({sigma_hi})")
+        self.guider = instantiate_from_config(guider_config)
+        inner = self.guider.image_guider if isinstance(self.guider, ActionCFG) else self.guider
+        if not isinstance(self.guider, self.GUIDERS) or not isinstance(inner, (VanillaCFG, LinearPredictionGuider)):
+            raise ValueError(f"IntervalCFG wraps VanillaCFG, LinearPredictionGuider, TrianglePredictionGuider or ActionCFG "
+                             f"over one of the first three; got {type(self.guider).__name__}")
+        self.additional_cond_keys = list(self.guider.additional_cond_keys)
+
+    def guided(self, sigma) -> bool:
+        """Whether the step at ``sigma`` (a number, or the step's per-row sigma tensor) is guided."""
+        s = float(sigma.reshape(-1)[0]) if isinstance(sigma, torch.Tensor) else float(sigma)
+        return self.sigma_lo < s <= self.sigma_hi
+
+    def __call__(self, x, sigma):
+        return self.guider(x, sigma) if self.guided(sigma) else x
+
+    def prepare_inputs(self, x, s, c, cond_mask, uc):
+        if self.guided(s):
+            return self.guider.prepare_inputs(x, s, c, cond_mask, uc)
+        return x, s, {k: c[k] for k in c}, cond_mask
+
+    def scale_vector(self, num_frames):
+        return self.guider.scale_vector(num_frames)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -369,9 +412,10 @@ class EulerEDMSampler(BaseDiffusionSampler):
 
     def _fusable(self, denoiser: "B200Denoiser", cond, uc) -> bool:
         from .modules import B200Wrapper
-        guider = self.guider.image_guider if isinstance(self.guider, ActionCFG) else self.guider
+        guider = self.guider.guider if isinstance(self.guider, IntervalCFG) else self.guider
+        guider = guider.image_guider if isinstance(guider, ActionCFG) else guider
         return (isinstance(denoiser.network, B200Wrapper) and isinstance(denoiser.denoiser.scaling, VScalingWithEDMcNoise)
-                and isinstance(guider, (VanillaCFG, LinearPredictionGuider))
+                and (isinstance(guider, (VanillaCFG, LinearPredictionGuider)) or type(self.guider) is IdentityGuider)
                 and all(k in cond for k in ("crossattn", "vector", "concat")))
 
 

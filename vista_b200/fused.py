@@ -4,7 +4,10 @@ Per step: ``sampler_prepare`` (cond-frame re-imposition, c_in scaling, CFG batch
 c_noise) -> UNet executor -> ``sampler_update`` (preconditioning, guidance, Euler step) or
 ``sampler_update_2m`` (the same denoised value, then the 2M step from the host's coefficient table).  Under action
 guidance (``diffusion.ActionCFG``) a second, T-row forward runs the conditional half of the prepared batch under the
-action-free conditioning, and ``sampler_update_action`` combines the three denoised values.  All state
+action-free conditioning, and ``sampler_update_action`` combines the three denoised values.  A step that is not guided
+(``diffusion.IntervalCFG`` outside its interval, ``IdentityGuider``) runs only the conditional half of the prepared batch
+through a T-row forward, then ``sampler_update_cond``; the host knows the schedule and replays each step's kind of graph.
+All state
 lives in persistent device buffers, the step index and sigma table are read on the device, so one
 step is a fixed launch sequence that is captured once in a CUDA graph and replayed (no host
 synchronisation inside the loop; the reference has two per step: sampling.py:102,109).
@@ -25,6 +28,7 @@ from .unet import padded_input_rows
 
 USE_GRAPH = os.environ.get("VISTA_B200_GRAPH", "1") != "0"
 USE_TAPE = os.environ.get("VISTA_B200_TAPE", "1") != "0"     # launch-tape replay of steps that hold collectives
+COND_SLOT = "cond"     # the runtime's conditioning slot of the unguided steps' N rows (UNetRuntime.set_conditioning)
 
 
 class _LoopState:
@@ -116,6 +120,12 @@ class _LoopState:
         self.net_img = rt.forward(self.unet_in[N * h * w:], self.c_noise[N:], self.mask2[N:], h, w)
         return self.net_img
 
+    def _forward_cond(self, rt):
+        """An unguided step's network call: the conditional half of the prepared batch through an N-row forward under
+        the runtime's conditioning of the full ``c`` (its own slot, beside action guidance's action-free N rows)."""
+        N, h, w = self.N, self.h, self.w
+        return rt.forward(self.unet_in[N * h * w:], self.c_noise[N:], self.mask2[N:], h, w, slot=COND_SLOT)
+
     def enable_action(self):
         """Allocates the per-frame action scale (once per state)."""
         if self.action_scales is None:
@@ -155,17 +165,23 @@ class _LoopState:
             pp = self.pair_peer
             ops.peer_put(pp["ack_src"], 16, 1, 16, pp["ack_dst"], 16, pp["ack_flag_remote"], 1, pp["c_ack_put"], pp["t_ack"], "cfg ack")
 
-    def one_step(self, rt, num_steps: int, multistep: bool = False, action: bool = False):
+    def one_step(self, rt, num_steps: int, multistep: bool = False, action: bool = False, guided: bool = True):
         self._prepare()
+        if not guided:
+            ops._sampler_update_cond(self.x, self._forward_cond(rt), self.cond_frame, self.mask,
+                                    self.coefs if multistep else None, self.d_prev if multistep else None, self.sigmas,
+                                    self.step, num_steps, self.N, self.h, self.w)
+            return
         net_out = self._forward(rt)
         self._finish(net_out, num_steps, multistep, self._forward_img(rt) if action else None)
 
-    def runner(self, rt, num_steps: int, multistep: bool = False, action: bool = False):
-        """Callable advancing one step the fastest supported way; call after one eager step (which allocates every
-        buffer of the executor).  Without a collective inside the UNet the launch sequence is replayed from a CUDA
-        graph: the whole step, or prepare + UNet in CFG-split mode (the pair exchange and the update stay eager)."""
+    def runner(self, rt, num_steps: int, multistep: bool = False, action: bool = False, guided: bool = True):
+        """Callable advancing one step the fastest supported way; call after one eager step of the same kind (which
+        allocates every buffer of the executor).  Without a collective inside the UNet the launch sequence is replayed
+        from a CUDA graph: the whole step, or prepare + UNet in CFG-split mode (the pair exchange and the update stay
+        eager)."""
         if not USE_GRAPH:
-            return lambda: self.one_step(rt, num_steps, multistep, action)
+            return lambda: self.one_step(rt, num_steps, multistep, action, guided)
         # NB: `rt.group is None` also names the DEFAULT process group; the runtime says whether its step holds collectives
         if getattr(rt, "has_collectives", False) and not USE_TAPE:
             return lambda: self.one_step(rt, num_steps, multistep, action)
@@ -183,7 +199,10 @@ class _LoopState:
                 else:
                     _lib.replay(self.tape)
             return run_taped
-        key = (num_steps, multistep, True) if action else (num_steps, multistep)
+        if not guided:
+            key = (num_steps, multistep, COND_SLOT)
+        else:
+            key = (num_steps, multistep, True) if action else (num_steps, multistep)
         if key in self.graphs:
             self.graph, self.graph_steps = self.graphs[key], key
         if self.graph is None or self.graph_steps != key:
@@ -192,7 +211,7 @@ class _LoopState:
             whole = self.split is None or self.pair_peer is not None      # no host-side collective in the step
             with torch.cuda.graph(g):             # capture does not execute
                 if whole:
-                    self.one_step(rt, num_steps, multistep, action)
+                    self.one_step(rt, num_steps, multistep, action, guided)
                 else:
                     self._prepare()
                     self._fwd_out = self._forward(rt)
@@ -223,13 +242,18 @@ def fused_sample(sampler, den, x: torch.Tensor, cond: Dict, uc: Optional[Dict], 
     dev = x.device
     N, zc, h, w = x.shape
     assert zc == 4 and N % T == 0
-    from .diffusion import ActionCFG, DPMPP2MSampler, dpmpp2m_coefficients
+    from .diffusion import ActionCFG, DPMPP2MSampler, IdentityGuider, IntervalCFG, dpmpp2m_coefficients
     multistep = isinstance(sampler, DPMPP2MSampler)
-    action = isinstance(sampler.guider, ActionCFG)
+    interval = sampler.guider if isinstance(sampler.guider, IntervalCFG) else None
+    guider = interval.guider if interval is not None else sampler.guider
+    action = isinstance(guider, ActionCFG)
+    identity = isinstance(guider, IdentityGuider)
     if multistep and getattr(net, "frame_sharded", False):
         raise NotImplementedError("DPMPP2MSampler: the frame-sharded fused loop runs the Euler sampler only")
     if action and getattr(net, "frame_sharded", False):
         raise NotImplementedError("ActionCFG: the frame-sharded fused loop runs one guidance scale only")
+    if (interval is not None or identity) and getattr(net, "frame_sharded", False):
+        raise NotImplementedError(f"{type(sampler.guider).__name__}: the frame-sharded fused loop guides every step")
     rt = net._rt_get(net.diffusion_model, T, dev)
     if getattr(net, "frame_sharded", False):
         return _fused_sample_sharded(sampler, rt, x, cond, uc, cond_frame, cond_mask, n, T, net)
@@ -257,18 +281,33 @@ def fused_sample(sampler, den, x: torch.Tensor, cond: Dict, uc: Optional[Dict], 
     st.mask2.copy_(torch.cat([st.mask, st.mask]))
     st.concat_u.copy_(_expand(uc["concat"], N, T))
     st.concat_c.copy_(_expand(cond["concat"], N, T))
-    sv = sampler.guider.scale_vector(T).to(dev, torch.float32)
-    st.scales.copy_(sv.repeat(N // T))
-    context = torch.cat((_expand(uc["crossattn"], N, T), _expand(cond["crossattn"], N, T)), 0)
-    y = torch.cat((_expand(uc["vector"], N, T), _expand(cond["vector"], N, T)), 0)
-    rt.set_conditioning(context, y)
-    if action:
-        st.enable_action()
-        st.action_scales.copy_(sampler.guider.action_scale_vector(T).to(dev, torch.float32).repeat(N // T))
-        st.img_cond = (_expand(sampler.guider.action_free(cond)["crossattn"], N, T), y[N:])
-        rt.set_conditioning(*st.img_cond)
+    # which steps are guided, from the fp32 sigma table the kernels read; only the kinds of step that run are conditioned
+    if identity:
+        schedule = [False] * n
+    elif interval is not None:
+        schedule = [interval.guided(sigmas[i]) for i in range(n)]
+    else:
+        schedule = [True] * n
+    if any(schedule):
+        sv = guider.scale_vector(T).to(dev, torch.float32)
+        st.scales.copy_(sv.repeat(N // T))
+        context = torch.cat((_expand(uc["crossattn"], N, T), _expand(cond["crossattn"], N, T)), 0)
+        y = torch.cat((_expand(uc["vector"], N, T), _expand(cond["vector"], N, T)), 0)
+        rt.set_conditioning(context, y)
+        if action:
+            st.enable_action()
+            st.action_scales.copy_(guider.action_scale_vector(T).to(dev, torch.float32).repeat(N // T))
+            st.img_cond = (_expand(guider.action_free(cond)["crossattn"], N, T), y[N:])
+            rt.set_conditioning(*st.img_cond)
+    if not all(schedule):
+        rt.set_conditioning(_expand(cond["crossattn"], N, T), _expand(cond["vector"], N, T), slot=COND_SLOT)
+    if getattr(net, "_cond_cache", None) is not None:
+        net._cond_cache = None      # the wrapper's own forward must set its conditioning again: this loop replaced it
 
-    _run_steps(st, rt, n, multistep, action)
+    if all(schedule):
+        _run_steps(st, rt, n, multistep, action)
+    else:
+        _run_schedule(st, rt, n, multistep, action, schedule)
     x.copy_(st.x)
     return x
 
@@ -282,6 +321,22 @@ def _run_steps(st: _LoopState, rt, n: int, multistep: bool = False, action: bool
     step = st.runner(rt, n, multistep, action)
     for _ in range(n - 1):
         step()
+
+
+def _run_schedule(st: _LoopState, rt, n: int, multistep: bool, action: bool, schedule):
+    """The steps of a schedule with unguided steps: schedule[i] says whether step i is guided.  The first step of each
+    kind runs eagerly, which allocates every buffer of the executor that kind of step uses; later ones replay its graph."""
+    if n < 3:
+        for guided in schedule:
+            st.one_step(rt, n, multistep, action, guided)
+        return
+    seen = set()
+    for guided in schedule:
+        if guided not in seen:
+            seen.add(guided)
+            st.one_step(rt, n, multistep, action, guided)
+        else:
+            st.runner(rt, n, multistep, action, guided)()
 
 
 def _fused_sample_sharded(sampler, rt, x, cond, uc, cond_frame, cond_mask, n: int, T: int, net=None) -> torch.Tensor:

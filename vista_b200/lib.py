@@ -133,6 +133,7 @@ SIGNATURES = {
     "b200v_sampler_update": [_P, _P, _I64, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P],
     "b200v_sampler_update_2m": [_P, _P, _I64, _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P],
     "b200v_sampler_update_action": [_P, _P, _I64, _P, _I64, _P, _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P],
+    "b200v_sampler_update_cond": [_P, _P, _I64, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P],
     "b200v_softmax_rows": [_P, _I64, _P, _I64, _I64, _I32, _P],
     "b200v_time_mix_small": [_P, _I64, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _P],
     "b200v_time_mix_small_u8": [_P, _I64, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P],

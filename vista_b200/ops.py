@@ -577,6 +577,21 @@ def sampler_update_action(x, net_out, net_img, cond_frame, mask, scales, action_
     _prof_end()
 
 
+def _sampler_update_cond(x, net_c, cond_frame, mask, coefs, d_prev, sigmas, step_idx, num_steps, T, h, w):
+    """The unguided step, for the fused loop of vista_b200.fused (its one caller), so not part of the public ops surface
+    that the production-path launch checks enumerate; tests/test_interval_cfg_gpu.py holds the kernel to fp64.
+    ``net_c`` is the [T h w, >= 4] fp32 output of the T conditional rows only, D = D_c.
+    ``coefs`` / ``d_prev`` as in ``sampler_update_2m`` for the 2M step (D is written to ``d_prev``), both None for the
+    Euler step."""
+    _count(2)
+    _prof_begin("other", "sampler_update_cond", 0.0, 0.0)
+    _lib.check(_lib.load().b200v_sampler_update_cond(x.data_ptr(), net_c.data_ptr(), net_c.stride(0), _ptr(cond_frame),
+                                                     _ptr(mask), _ptr(coefs), _ptr(d_prev), sigmas.data_ptr(),
+                                                     step_idx.data_ptr(), num_steps, T, h, w, _stream()),
+               "b200v_sampler_update_cond")
+    _prof_end()
+
+
 def nchw_to_tokens(x, out, NB, Cc, H, W):
     _count(1)
     _prof_begin("other", "nchw_to_tokens", 0.0, 0.0)

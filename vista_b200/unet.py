@@ -225,12 +225,15 @@ class UNetRuntime:
         self.gemm(v, W["out"], out)
         return out
 
-    def set_conditioning(self, context: torch.Tensor, y: torch.Tensor):
+    def set_conditioning(self, context: torch.Tensor, y: torch.Tensor, slot: str = ""):
         """context (B,1,3456) / y (B,768): everything that does not depend on sigma or the step.  One conditioning is
         kept per batch size B (its constants are buffers of B rows), so that the CFG pair's 2T rows and action guidance's
-        T image rows are conditioned side by side; setting B again replaces only B's."""
+        T image rows are conditioned side by side; setting B again replaces only B's.  A named ``slot`` keeps one more
+        conditioning of B rows in buffers of its own, which ``forward(..., slot=slot)`` reads: the unguided steps of
+        interval guidance condition their T rows on the full ``c`` beside action guidance's action-free T rows."""
         T = self.T
         B = context.shape[0]
+        p = f"{slot}." if slot else ""
         # both cross-attentions are folded to per-frame constants, which is exact for ONE key token only
         # (encoders/modules.py:514-516, video_attention.py:256-257): refuse anything else instead of using token 0
         from .spec import ACTION_DIM
@@ -241,18 +244,18 @@ class UNetRuntime:
         ctx16.copy_(context.reshape(B, -1))
         y16 = self.buf("cond.y", B, y.shape[-1])
         y16.copy_(y)
-        cond = dict(B=B, label=self._mlp(y16, *self.label_emb, "label"), sp={}, tm={}, pos={})
+        cond = dict(B=B, label=self._mlp(y16, *self.label_emb, p + "label"), sp={}, tm={}, pos={})
         tctx16 = self.buf("cond.tctx", B // T, ctx16.shape[1])
         tctx16.copy_(ctx16[::T])                                   # video_attention.py:256
         frames = torch.arange(T, dtype=torch.float32, device=self.dev)
         for t in self.plan.transformers():
             L = self.layers[t.prefix]
-            cond["sp"][t.prefix] = self._attn2_const(L["attn2"], ctx16, f"cond.sp.{t.prefix}")
-            cond["tm"][t.prefix] = self._attn2_const(L["tattn2"], tctx16, f"cond.tm.{t.prefix}")
+            cond["sp"][t.prefix] = self._attn2_const(L["attn2"], ctx16, f"{p}cond.sp.{t.prefix}")
+            cond["tm"][t.prefix] = self._attn2_const(L["tattn2"], tctx16, f"{p}cond.tm.{t.prefix}")
             temb = self.buf("cond.temb", T, t.ch)
             ops.timestep_embedding(frames, temb, t.ch)
-            cond["pos"][t.prefix] = self._mlp(temb, *L["pos"], f"cond.pos.{t.prefix}")
-        self.cond = self.conds[B] = cond
+            cond["pos"][t.prefix] = self._mlp(temb, *L["pos"], f"{p}cond.pos.{t.prefix}")
+        self.cond = self.conds[(B, slot) if slot else B] = cond
 
     # ------------------------------------------------------------------ layers
     def _fuse_stats(self, B, h, w) -> bool:
@@ -345,14 +348,15 @@ class UNetRuntime:
 
     # ------------------------------------------------------------------ forward
     def forward(self, x_tokens: torch.Tensor, c_noise: torch.Tensor, cond_mask: Optional[torch.Tensor],
-                h: int, w: int, net_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                h: int, w: int, net_out: Optional[torch.Tensor] = None, slot: str = "") -> torch.Tensor:
         """x_tokens: [(B h w), 8] fp16 (x*c_in | concat), either contiguous or a view of zero-padded IN_PAD-wide rows
         (padded_input_rows); c_noise: [B] fp32; returns [(B h w), 8] fp32 whose first out_channels columns are the
-        network output."""
+        network output.  ``slot``: which conditioning of B rows to use (set_conditioning)."""
         cfg, T = self.cfg, self.T
         B = c_noise.numel()
-        assert B in self.conds, f"call set_conditioning() with {B} rows first"
-        self.cond = self.conds[B]
+        ckey = (B, slot) if slot else B
+        assert ckey in self.conds, f"call set_conditioning() with {B} rows first" + (f" (slot {slot!r})" if slot else "")
+        self.cond = self.conds[ckey]
         assert B % T == 0 and x_tokens.shape[0] == B * h * w
         mc, ed = cfg.model_channels, cfg.time_embed_dim
         # GroupNorm statistics / scratch are persistent per batch size (never replaced or freed): CUDA graphs and launch
