@@ -9,6 +9,7 @@ Mirrors (paths relative to the reference root):
   VanillaCFG / Identity / Linear / TrianglePredictionGuider ... guiders.py
   ActionCFG ................ a separate guidance scale for the action (not in Vista; InstructPix2Pix's two-scale CFG)
   IntervalCFG .............. guidance on a sigma interval only (not in Vista; Kynkäänniemi et al. 2024)
+  cache_schedule ........... which steps run the whole UNet under feature caching (not in Vista; Ma et al. 2024)
   EulerEDMSampler .......... vwm/modules/diffusionmodules/sampling.py:15-124
   DPMPP2MSampler ........... sgm's sampling.py DPMPP2MSampler (Vista does not ship it), on the same loop
   instantiate_from_config .. vwm/util.py:154-173
@@ -312,6 +313,31 @@ class IntervalCFG(Guider):
 
 
 # ----------------------------------------------------------------------------------------------
+# feature caching
+# ----------------------------------------------------------------------------------------------
+def _check_cache_args(cache_interval, cache_branch):
+    for name, v, lo in (("cache_interval", cache_interval, 1), ("cache_branch", cache_branch, 0)):
+        if isinstance(v, bool) or not isinstance(v, int) or v < lo:
+            raise ValueError(f"{name} must be an int >= {lo}; got {v!r}")
+
+
+def cache_schedule(kinds, interval: int) -> List[bool]:
+    """Feature caching (Ma et al. 2024, DeepCache, arXiv 2312.00858): which steps run the whole UNet (True) and which
+    reuse the deep feature of the last full step and run only the outermost blocks (False).  ``kinds[i]`` is step i's
+    kind of network call (guided or not, under IntervalCFG or IdentityGuider); a step is full if it is the first, if its
+    kind differs from step i-1's, or if ``interval`` steps have passed since the last full step.  A cached step reads the
+    feature its own kind's rows left, so a kind change always starts with a full step."""
+    _check_cache_args(interval, 0)
+    full, last = [], 0
+    for i, k in enumerate(kinds):
+        f = i == 0 or k != kinds[i - 1] or i - last >= interval
+        if f:
+            last = i
+        full.append(f)
+    return full
+
+
+# ----------------------------------------------------------------------------------------------
 # sampler
 # ----------------------------------------------------------------------------------------------
 class B200Denoiser:
@@ -347,13 +373,24 @@ def _unwrap_reference_closure(fn):
 
 
 class BaseDiffusionSampler:
+    """``cache_interval`` / ``cache_branch``: feature caching on the fused loop (``cache_schedule``).  With an interval
+    k > 1 a full UNet step runs at most every k steps, and the steps between run input blocks 0..b and output blocks
+    n-1-b..n-1 on the deep feature of the last full step, b = ``cache_branch``.  1 (the default) runs every step whole.
+    Only the fused loop caches: the torch loop, ``s_churn > 0`` and a frame-sharded engine raise NotImplementedError."""
+
     def __init__(self, discretization_config, num_steps: Optional[int] = None, guider_config=None,
-                 verbose: bool = False, device: str = "cuda"):
+                 verbose: bool = False, device: str = "cuda", cache_interval: int = 1, cache_branch: int = 0):
+        _check_cache_args(cache_interval, cache_branch)
         self.num_steps = num_steps
         self.discretization = instantiate_from_config(discretization_config)
         self.guider = instantiate_from_config(guider_config)
         self.verbose = verbose
         self.device = device
+        self.cache_interval, self.cache_branch = cache_interval, cache_branch
+
+    def _refuse_cache(self, why: str):
+        if self.cache_interval > 1:
+            raise NotImplementedError(f"{type(self).__name__}: cache_interval > 1 runs on the fused loop only, not {why}")
 
     def prepare_sampling_loop(self, x, cond, uc=None, num_steps=None):
         sigmas = self.discretization(self.num_steps if num_steps is None else num_steps, device=self.device)
@@ -395,9 +432,12 @@ class EulerEDMSampler(BaseDiffusionSampler):
 
     def __call__(self, denoiser, x, cond, uc=None, cond_frame=None, cond_mask=None, num_steps=None):
         denoiser = _unwrap_reference_closure(denoiser)
+        if self.s_churn > 0.0:
+            self._refuse_cache("with s_churn > 0")
         if isinstance(denoiser, B200Denoiser) and self.s_churn == 0.0 and self._fusable(denoiser, cond, uc):
             from .fused import fused_sample
             return fused_sample(self, denoiser, x, cond, uc, cond_frame, cond_mask, num_steps)
+        self._refuse_cache("on the torch loop")
         x, s_in, sigmas, num_sigmas, cond, uc = self.prepare_sampling_loop(x, cond, uc, num_steps)
         replace_cond_frames = cond_mask is not None and bool(cond_mask.any())
         for i in self.get_sigma_gen(num_sigmas):
@@ -454,6 +494,7 @@ class DPMPP2MSampler(BaseDiffusionSampler):
         if isinstance(denoiser, B200Denoiser) and self._fusable(denoiser, cond, uc):
             from .fused import fused_sample
             return fused_sample(self, denoiser, x, cond, uc, cond_frame, cond_mask, num_steps)
+        self._refuse_cache("on the torch loop")
         x, s_in, sigmas, num_sigmas, cond, uc = self.prepare_sampling_loop(x, cond, uc, num_steps)
         coefs = dpmpp2m_coefficients(sigmas).tolist()
         replace_cond_frames = cond_mask is not None and bool(cond_mask.any())

@@ -7,6 +7,8 @@ guidance (``diffusion.ActionCFG``) a second, T-row forward runs the conditional 
 action-free conditioning, and ``sampler_update_action`` combines the three denoised values.  A step that is not guided
 (``diffusion.IntervalCFG`` outside its interval, ``IdentityGuider``) runs only the conditional half of the prepared batch
 through a T-row forward, then ``sampler_update_cond``; the host knows the schedule and replays each step's kind of graph.
+Under feature caching (``cache_interval`` > 1, ``diffusion.cache_schedule``) a cached step is the same step with its
+network calls cut to the outermost blocks (``UNetRuntime.forward(..., cached=True)``); it has a graph of its own.
 All state
 lives in persistent device buffers, the step index and sigma table are read on the device, so one
 step is a fixed launch sequence that is captured once in a CUDA graph and replayed (no host
@@ -104,27 +106,36 @@ class _LoopState:
         ops.sampler_prepare(self.x, self.cond_frame, self.mask, self.concat_u, self.concat_c, self.sigmas, self.step,
                             self.unet_in, self.c_noise, self.N, self.h, self.w)
 
-    def _forward(self, rt):
+    def _forward(self, rt, cache=None):
+        """``cache``: the keywords of a cached forward (``_cache_kw``), or None for a full one."""
         N, h, w = self.N, self.h, self.w
         if self.split is None:
-            return rt.forward(self.unet_in, self.c_noise, self.mask2, h, w)
+            return rt.forward(self.unet_in, self.c_noise, self.mask2, h, w, **(cache or {}))
         half, rows = self.split[0], N * h * w
         out = self.net_full[half * rows:(half + 1) * rows] if self.pair_peer is not None else None   # straight into the exchange buffer
         return rt.forward(self.unet_in[half * rows:(half + 1) * rows], self.c_noise[half * N:(half + 1) * N],
                           self.mask2[half * N:(half + 1) * N], h, w, net_out=out)
 
-    def _forward_img(self, rt):
+    def _forward_img(self, rt, cache=None):
         """The action-free image branch: the conditional half of the prepared batch (rows bit for bit what the branch
         needs) through an N-row forward under the runtime's N-row conditioning."""
         N, h, w = self.N, self.h, self.w
-        self.net_img = rt.forward(self.unet_in[N * h * w:], self.c_noise[N:], self.mask2[N:], h, w)
+        self.net_img = rt.forward(self.unet_in[N * h * w:], self.c_noise[N:], self.mask2[N:], h, w, **(cache or {}))
         return self.net_img
 
-    def _forward_cond(self, rt):
+    def _forward_cond(self, rt, cache=None):
         """An unguided step's network call: the conditional half of the prepared batch through an N-row forward under
         the runtime's conditioning of the full ``c`` (its own slot, beside action guidance's action-free N rows)."""
         N, h, w = self.N, self.h, self.w
-        return rt.forward(self.unet_in[N * h * w:], self.c_noise[N:], self.mask2[N:], h, w, slot=COND_SLOT)
+        return rt.forward(self.unet_in[N * h * w:], self.c_noise[N:], self.mask2[N:], h, w, slot=COND_SLOT,
+                          **(cache or {}))
+
+    @staticmethod
+    def _cache_kw(cached: bool, cache_branch: int):
+        """The forward keywords of a step: none for a full step (the launches of an uncached loop), the branch for a
+        cached one.  The N-row forwards of ActionCFG's image branch and of unguided steps share their buffers; the cache
+        schedule never lets a cached step follow a full step of the other kind."""
+        return dict(cache_branch=cache_branch, cached=True) if cached else None
 
     def enable_action(self):
         """Allocates the per-frame action scale (once per state)."""
@@ -165,23 +176,27 @@ class _LoopState:
             pp = self.pair_peer
             ops.peer_put(pp["ack_src"], 16, 1, 16, pp["ack_dst"], 16, pp["ack_flag_remote"], 1, pp["c_ack_put"], pp["t_ack"], "cfg ack")
 
-    def one_step(self, rt, num_steps: int, multistep: bool = False, action: bool = False, guided: bool = True):
+    def one_step(self, rt, num_steps: int, multistep: bool = False, action: bool = False, guided: bool = True,
+                 cached: bool = False, cache_branch: int = 0):
+        """``cached``: run the step's network calls as cached forwards of branch ``cache_branch``; the update is the same."""
+        cache = self._cache_kw(cached, cache_branch)
         self._prepare()
         if not guided:
-            ops._sampler_update_cond(self.x, self._forward_cond(rt), self.cond_frame, self.mask,
+            ops._sampler_update_cond(self.x, self._forward_cond(rt, cache), self.cond_frame, self.mask,
                                     self.coefs if multistep else None, self.d_prev if multistep else None, self.sigmas,
                                     self.step, num_steps, self.N, self.h, self.w)
             return
-        net_out = self._forward(rt)
-        self._finish(net_out, num_steps, multistep, self._forward_img(rt) if action else None)
+        net_out = self._forward(rt, cache)
+        self._finish(net_out, num_steps, multistep, self._forward_img(rt, cache) if action else None)
 
-    def runner(self, rt, num_steps: int, multistep: bool = False, action: bool = False, guided: bool = True):
+    def runner(self, rt, num_steps: int, multistep: bool = False, action: bool = False, guided: bool = True,
+               cached: bool = False, cache_branch: int = 0):
         """Callable advancing one step the fastest supported way; call after one eager step of the same kind (which
         allocates every buffer of the executor).  Without a collective inside the UNet the launch sequence is replayed
         from a CUDA graph: the whole step, or prepare + UNet in CFG-split mode (the pair exchange and the update stay
         eager)."""
         if not USE_GRAPH:
-            return lambda: self.one_step(rt, num_steps, multistep, action, guided)
+            return lambda: self.one_step(rt, num_steps, multistep, action, guided, cached, cache_branch)
         # NB: `rt.group is None` also names the DEFAULT process group; the runtime says whether its step holds collectives
         if getattr(rt, "has_collectives", False) and not USE_TAPE:
             return lambda: self.one_step(rt, num_steps, multistep, action)
@@ -203,6 +218,8 @@ class _LoopState:
             key = (num_steps, multistep, COND_SLOT)
         else:
             key = (num_steps, multistep, True) if action else (num_steps, multistep)
+        if cached:
+            key = key + ("cached", cache_branch)
         if key in self.graphs:
             self.graph, self.graph_steps = self.graphs[key], key
         if self.graph is None or self.graph_steps != key:
@@ -211,7 +228,7 @@ class _LoopState:
             whole = self.split is None or self.pair_peer is not None      # no host-side collective in the step
             with torch.cuda.graph(g):             # capture does not execute
                 if whole:
-                    self.one_step(rt, num_steps, multistep, action, guided)
+                    self.one_step(rt, num_steps, multistep, action, guided, cached, cache_branch)
                 else:
                     self._prepare()
                     self._fwd_out = self._forward(rt)
@@ -254,9 +271,14 @@ def fused_sample(sampler, den, x: torch.Tensor, cond: Dict, uc: Optional[Dict], 
         raise NotImplementedError("ActionCFG: the frame-sharded fused loop runs one guidance scale only")
     if (interval is not None or identity) and getattr(net, "frame_sharded", False):
         raise NotImplementedError(f"{type(sampler.guider).__name__}: the frame-sharded fused loop guides every step")
+    cache_interval, cache_branch = sampler.cache_interval, sampler.cache_branch
+    if cache_interval > 1 and getattr(net, "frame_sharded", False):
+        raise NotImplementedError(f"{type(sampler).__name__}: the frame-sharded fused loop does not cache features")
     rt = net._rt_get(net.diffusion_model, T, dev)
     if getattr(net, "frame_sharded", False):
         return _fused_sample_sharded(sampler, rt, x, cond, uc, cond_frame, cond_mask, n, T, net)
+    if cache_interval > 1 and not cache_branch < len(rt.plan.input_blocks):
+        raise ValueError(f"cache_branch must be below the UNet's {len(rt.plan.input_blocks)} input blocks; got {cache_branch}")
     key = (N, h, w)
     states = rt.__dict__.setdefault("_loop_states", {})
     st: _LoopState = states.get(key)
@@ -304,7 +326,10 @@ def fused_sample(sampler, den, x: torch.Tensor, cond: Dict, uc: Optional[Dict], 
     if getattr(net, "_cond_cache", None) is not None:
         net._cond_cache = None      # the wrapper's own forward must set its conditioning again: this loop replaced it
 
-    if all(schedule):
+    if cache_interval > 1:
+        from .diffusion import cache_schedule
+        _run_schedule(st, rt, n, multistep, action, schedule, cache_schedule(schedule, cache_interval), cache_branch)
+    elif all(schedule):
         _run_steps(st, rt, n, multistep, action)
     else:
         _run_schedule(st, rt, n, multistep, action, schedule)
@@ -323,20 +348,23 @@ def _run_steps(st: _LoopState, rt, n: int, multistep: bool = False, action: bool
         step()
 
 
-def _run_schedule(st: _LoopState, rt, n: int, multistep: bool, action: bool, schedule):
-    """The steps of a schedule with unguided steps: schedule[i] says whether step i is guided.  The first step of each
-    kind runs eagerly, which allocates every buffer of the executor that kind of step uses; later ones replay its graph."""
+def _run_schedule(st: _LoopState, rt, n: int, multistep: bool, action: bool, schedule, full=None, cache_branch: int = 0):
+    """The steps of a schedule with unguided or cached steps: schedule[i] says whether step i is guided, full[i] (None:
+    every step) whether it runs the whole UNet.  The first step of each kind runs eagerly, which allocates every buffer
+    of the executor that kind of step uses; later ones replay its graph."""
+    kinds = [(g, True if full is None else f) for g, f in zip(schedule, full or schedule)]
     if n < 3:
-        for guided in schedule:
-            st.one_step(rt, n, multistep, action, guided)
+        for guided, whole in kinds:
+            st.one_step(rt, n, multistep, action, guided, not whole, cache_branch)
         return
     seen = set()
-    for guided in schedule:
-        if guided not in seen:
-            seen.add(guided)
-            st.one_step(rt, n, multistep, action, guided)
+    for kind in kinds:
+        guided, whole = kind
+        if kind not in seen:
+            seen.add(kind)
+            st.one_step(rt, n, multistep, action, guided, not whole, cache_branch)
         else:
-            st.runner(rt, n, multistep, action, guided)()
+            st.runner(rt, n, multistep, action, guided, not whole, cache_branch)()
 
 
 def _fused_sample_sharded(sampler, rt, x, cond, uc, cond_frame, cond_mask, n: int, T: int, net=None) -> torch.Tensor:

@@ -59,6 +59,8 @@ class UNetRuntime:
         self._sd = None
         self.cond = None
         self.conds: Dict[int, dict] = {}      # batch size -> its conditioning; forward(B rows) uses conds[B]
+        # (B, h, w) -> per output block, whether the last full forward left GroupNorm partials of its input's h half
+        self._h_filled: Dict[Tuple[int, int, int], List[bool]] = {}
 
     # ------------------------------------------------------------------ weight packing
     def _f32(self, name):
@@ -348,12 +350,24 @@ class UNetRuntime:
 
     # ------------------------------------------------------------------ forward
     def forward(self, x_tokens: torch.Tensor, c_noise: torch.Tensor, cond_mask: Optional[torch.Tensor],
-                h: int, w: int, net_out: Optional[torch.Tensor] = None, slot: str = "") -> torch.Tensor:
+                h: int, w: int, net_out: Optional[torch.Tensor] = None, slot: str = "", cache_branch: int = 0,
+                cached: bool = False) -> torch.Tensor:
         """x_tokens: [(B h w), 8] fp16 (x*c_in | concat), either contiguous or a view of zero-padded IN_PAD-wide rows
         (padded_input_rows); c_noise: [B] fp32; returns [(B h w), 8] fp32 whose first out_channels columns are the
-        network output.  ``slot``: which conditioning of B rows to use (set_conditioning)."""
+        network output.  ``slot``: which conditioning of B rows to use (set_conditioning).
+
+        ``cached`` (feature caching, Ma et al. 2024, DeepCache): run input blocks 0..b and output blocks n-1-b..n-1 only,
+        b = ``cache_branch``.  Output block n-1-b reads the h half of its skip-concat buffer, and that half's GroupNorm
+        column partials, as the last full forward of B rows at (h, w) left them: the feature is never copied, and a cached
+        forward launches a subsequence of the full forward's launches."""
         cfg, T = self.cfg, self.T
         B = c_noise.numel()
+        if cached:
+            n_in = len(self.plan.input_blocks)
+            if not 0 <= cache_branch < n_in or len(self.plan.output_blocks) != n_in:
+                raise ValueError(f"cache_branch must be in [0, {n_in - 1}]; got {cache_branch}")
+            if (B, h, w) not in self._h_filled:
+                raise RuntimeError(f"a cached forward of {B} rows at {h} x {w} needs a full forward of them first")
         ckey = (B, slot) if slot else B
         assert ckey in self.conds, f"call set_conditioning() with {B} rows first" + (f" (slot {slot!r})" if slot else "")
         self.cond = self.conds[ckey]
@@ -443,17 +457,25 @@ class UNetRuntime:
         cur, cur_p = x_tokens, None
         hh, ww = h, w                      # size of the tensor entering the block
         for i, blk in enumerate(plan.input_blocks):
+            if cached and i > cache_branch:
+                break
             j = n_out - 1 - i
             dp = cat_parts[j][:, ch_in_h[j]:] if cat_parts[j] is not None else None
             cur, cat_ok[j][1] = run_block(blk, cur, cat_bufs[j][:, ch_in_h[j]:], hh, ww, xp=cur_p, dp=dp)
             cur_p = dp if cat_ok[j][1] else None
             hh, ww = in_sizes[i]
         # --- middle block -> h slice of output block 0
-        dp = cat_parts[0][:, :ch_in_h[0]] if cat_parts[0] is not None else None
-        cur, cat_ok[0][0] = run_block(plan.middle_block, cur, cat_bufs[0][:, :ch_in_h[0]], hh, ww, xp=cur_p, dp=dp)
+        j0 = n_out - 1 - cache_branch if cached else 0
+        if cached:       # the h half of cat{j0} and its partials are the last full forward's: whether those were filled
+            cat_ok[j0][0] = self._h_filled[(B, h, w)][j0]
+        else:
+            dp = cat_parts[0][:, :ch_in_h[0]] if cat_parts[0] is not None else None
+            cur, cat_ok[0][0] = run_block(plan.middle_block, cur, cat_bufs[0][:, :ch_in_h[0]], hh, ww, xp=cur_p, dp=dp)
         # --- output blocks
         last_p = None
         for j, blk in enumerate(plan.output_blocks):
+            if j < j0:
+                continue
             bh, bw = sizes[j]
             if j + 1 < n_out:
                 dst = cat_bufs[j + 1][:, :ch_in_h[j + 1]]
@@ -468,6 +490,8 @@ class UNetRuntime:
                 cat_ok[j + 1][0] = ok
             else:
                 last_p = dp if ok else None
+        if not cached:
+            self._h_filled[(B, h, w)] = [ok[0] for ok in cat_ok]
         # --- out: GroupNorm32 -> SiLU -> conv3x3(320 -> 4)                      (video_model.py:434-440,502-503)
         M = B * h * w
         a = self._gn(cur, self.buf("out.a", M, mc), B, h * w, self.out_norm, 1e-5, True, self.out_gn_idx, part=last_p)
